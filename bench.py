@@ -1,12 +1,16 @@
 #!/usr/bin/env python
-"""bench.py -- QPS of the HNSW candidate-scoring path on B200 (BASELINE.json metric).
+"""bench.py -- QPS of the HNSW candidate-scoring path on one H100 (BASELINE.json metric).
 
 Workload (BASELINE.json configs[2], the configuration the metric is quoted on):
     dims=768, N=1M synthetic fp32 vectors (clustered mixture, L2-normalised), cosine `<=>`,
     hnsw(m=32, efconstruction=200, efsearch=64); a *step* = one batch of `--batch` k-NN queries
     (k = efsearch = 64) through the search path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
+
+`--steps` is the number of timed steps of the headline and of every leg's timed loop.  `--dump-outputs DIR` writes what the
+last timed headline step returned to its caller (labels, result counts, per-query counters; float64) as DIR/<name>.npy: with
+the same arguments the inputs are identical from run to run, so two builds can be compared output for output.
 
 Our arm     : the CUDA path.  `value` = queries/s with the query batch already resident in HBM
               (pgemb_search_batch_device on torch's stream, CUDA-event timed, max over ranks);
@@ -27,10 +31,10 @@ N>1 (`torchrun`): the index (3.3 GB) fits one GPU, so ranks hold replicas and sp
 (SURVEY.md section 8(e)): no data-path collective, "scaling": "weak" (per-GPU batch fixed).
 
 Besides the headline, the ONE JSON line carries legs for the other BASELINE configurations, each with its own in-run parity
-check against the compiled reference (untimed) -- so that the driver's records hold evidence for them too:
+check against the compiled reference (untimed):
   "configs1"   (N=1)  configs[1]: dims 128, N 100K, L2, m 16 -- a 51 MB working set that lives in L2 (bound stated as such);
   "scan_topk"  (N=1)  the brute-force operator path (SURVEY.md 8(f3) / K6): 1024 queries x the 1M x 768 table through the
-                      tcgen05 tensor-core filter + exact re-scoring, TF/s against the TF32 roof, parity against the exact kernels;
+                      wgmma tensor-core filter + exact re-scoring, TF/s against the TF32 roof, parity against the exact kernels;
   "sharded"    (N>1)  configs[3] shape: dims 1536, L2, m 32, id-range shards of PGEMB_BENCH_SHARD_ROWS (1.25M) rows per GPU
                       (10M rows at 8 GPUs), every query searched on every shard, exchange + merge INSIDE the timed region --
                       peers' lists read over NVLink by the wait+merge kernel (no collective) and, for comparison, ONE NCCL
@@ -74,6 +78,8 @@ def parse():
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="target CPU time of the cpu_baseline sample")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (development)")
     ap.add_argument("--no-legs", action="store_true", help="headline only: skip the configs1 / scan_topk / sharded legs (development)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed headline step as DIR/<name>.npy (float64)")
     return ap.parse_args()
 
 
@@ -118,9 +124,9 @@ def gen_points_raw(torch, n, seed, centres, chunk=1 << 16):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / power limit / throttle reasons during the timed region (read-only queries)."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
-        "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+        "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, gpu_index):
         self.rows, self.proc = [], None
@@ -138,45 +144,25 @@ class ClockSampler:
 
     def stop(self):
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
-        sm, mx, reasons = [], None, set()
+        self.proc.wait()
+        sm, mx, plim, reasons = [], None, None, set()
         for r in self.rows:
             f = [x.strip() for x in r.split(",")]
-            if len(f) < 7:
+            if len(f) < 8:
                 continue
             try:
                 sm.append(float(f[0]))
                 mx = float(f[1])
+                plim = float(f[7])
             except ValueError:
                 continue
             for name, val in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[3:7]):
                 if val.lower().startswith("active"):
                     reasons.add(name)
-        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm)}
-
-
-def ncu_traffic_bytes(batch):
-    """DRAM read+write bytes of one traversal launch from the committed ncu --set full capture (profiles/; the newest round's),
-    valid for the default 32768-query launch of this workload only; (None, None) otherwise."""
-    if batch != 32768:
-        return None, None
-    scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9, "Tbyte": 1e12}
-    for name in ("r2_search_kernel_cosine768_metrics.csv", "r1_search_kernel_cosine768_metrics.csv"):
-        p = os.path.join(ROOT, "profiles", name)
-        if not os.path.isfile(p):
-            continue
-        tot = 0.0
-        try:
-            for line in open(p):
-                f = line.strip().split(",")
-                if len(f) >= 4 and f[-3] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                    tot += float(f[-1]) * scale.get(f[-2], 1.0)
-        except Exception:
-            continue
-        if tot > 0:
-            return int(tot), name
-    return None, None
+        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": mx, "power_limit_w": plim, "reasons": sorted(reasons),
+                "samples": len(sm)}
 
 
 def measured_peak_gbs():
@@ -186,7 +172,27 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
+
+
+def peak_tf32_tflops():
+    """Dense TF32 tensor rate to compare the scan legs against: half the measured BF16 rate if MEASURED_PEAKS.json has one,
+    else the H100 SXM data sheet's 495 TFLOP/s (for a card allowed 700 W)."""
+    try:
+        return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"]) / 2.0, "MEASURED_PEAKS.json bf16_tflops / 2"
+    except Exception:
+        return 495.0, "H100 SXM data sheet (dense TF32), not measured"
+
+
+def dump_outputs(out_dir, arrays):
+    """The arrays a caller of the timed path received, as float64 .npy files (all values here are exact in float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a, dtype=np.float64)
+        total += a.nbytes
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+    assert total <= 64 << 20, f"--dump-outputs wrote {total} bytes"
 
 
 def protect_stdout():
@@ -280,6 +286,11 @@ def main():
         torch.cuda.profiler.stop()
     ms = ev0.elapsed_time(ev1)
     launches = int(lib.pgemb_launch_count()) - launches0
+    if args.dump_outputs:
+        # the last timed step's results, before anything below reuses the output buffers
+        sfx = f"_rank{rank}" if world > 1 else ""
+        dump_outputs(args.dump_outputs, {f"labels{sfx}": d_lab.cpu().numpy().view(np.uint64), f"n_results{sfx}": d_nres[K - 1].cpu().numpy(),
+                                         f"stats{sfx}": d_stats[K - 1].cpu().numpy()})
     clocks = sampler.stop()
     tms = torch.tensor([ms], device="cuda")
     if world > 1:
@@ -295,11 +306,9 @@ def main():
     kms = ms / K                                                                       # this rank's launches (CUDA events on the launching stream)
     peak, peak_src = measured_peak_gbs()
     achieved = alg_bytes / (kms * 1e-3) / 1e9
-    traffic, traffic_file = ncu_traffic_bytes(B) if n == 1_000_000 else (None, None)
     roofline = {"bound": "hbm", "kernel": "search_kernel<cosine> (K3: TMA row gather + exact distance + queue update)",
                 "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 4),
-                "peak_source": peak_src, "traffic": traffic,
-                "traffic_source": f"static: profiles/{traffic_file} (ncu --set full capture of this launch shape; not re-measured in this run)" if traffic else None,
+                "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": round(kms, 3), "kernel_ms_source": "timed region / steps (one launch per step)",
                 "per_query": {"dist_evals": float(st[:, 0].mean()), "expansions": float(st[:, 1].mean()),
                               "bytes": float(alg_bytes / B)}}
@@ -380,11 +389,11 @@ def main():
             "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": round(ms_max / K, 3), "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload, "queries_per_step": B, "queries_per_step_per_gpu": B, "k": ef, "parallelism": f"replicas x{world}, queries split",
-                       "l2": "inputs larger than L2 (3.3 GB index vs 126 MB L2); distinct queries every step",
+                       "l2": "inputs larger than L2 (3.3 GB index vs 50 MB L2); distinct queries every step",
                        "graph": f"GPU bulk build (batch<={args.build_batch}), {build_s:.1f}s, shared by both arms",
                        "distribution": "mixture of sqrt(N) Gaussians, noise 0.3x inter-centre spacing, L2-normalised; seeds 1234/5678"},
             "recall_at_10": round(recall, 4),
-            "e2e": e2e, "gpu_launches": launches, "clocks": clocks, "roofline": roofline,
+            "gpu": torch.cuda.get_device_name(local), "e2e": e2e, "gpu_launches": launches, "clocks": clocks, "roofline": roofline,
             "cpu_baseline": cpu_baseline, "parity": parity,
         }
         out.update(legs)
@@ -418,7 +427,7 @@ def leg_scan_topk(args, torch, lib, _lib, idx, X, Q, n):
     os.environ.pop("PGEMB_SCAN_TC", None)
     run(q, lab, dd, nn)                                            # warm-up: staging buffers, norms
     c0 = scan_counters(lib)
-    reps, times = 3, []
+    reps, times = args.steps, []
     for _ in range(reps):
         torch.cuda.synchronize()
         t0 = time.perf_counter()
@@ -436,18 +445,14 @@ def leg_scan_topk(args, torch, lib, _lib, idx, X, Q, n):
     os.environ.pop("PGEMB_SCAN_TC", None)
     same = bool(lab[:ns].tobytes() == l2.tobytes() and dd[:ns].tobytes() == d2.tobytes() and nn[:ns].tolist() == n2.tolist())
     flops = 2.0 * nq * n * DIMS
-    try:
-        bf16 = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"])
-    except Exception:
-        bf16 = 1590.0
-    peak_tf32 = bf16 / 2.0
+    peak_tf32, peak_src = peak_tf32_tflops()
     hbm, _ = measured_peak_gbs()
     table_bytes = n * DIMS * 4
     qtiles = (nq + 127) // 128
     return {"workload": f"pgemb_scan_topk: {nq} queries x {n} rows x {DIMS} dims, cosine, k={k} (exact brute-force k-NN, SURVEY.md 8(f3))",
             "seconds": round(t, 5), "pairs_per_s": round(nq * n / t, 0), "queries_per_s": round(nq / t, 1),
             "tensor": {"bound": "tensor", "achieved": round(flops / t / 1e12, 1), "peak": round(peak_tf32, 1), "unit": "TFLOP/s",
-                       "frac": round(flops / t / 1e12 / peak_tf32, 4), "peak_source": "MEASURED_PEAKS.json bf16_tflops / 2 (TF32 runs at half the bf16 rate)"},
+                       "frac": round(flops / t / 1e12 / peak_tf32, 4), "peak_source": peak_src},
             "hbm_bound_one_table_pass_per_query_tile_s": round(qtiles * table_bytes / (hbm * 1e9), 5),
             "x_of_that_bound": round(t / (qtiles * table_bytes / (hbm * 1e9)), 2),
             "rescored_fraction": round((c1["rescored"] - c0["rescored"]) / max(1, c1["pairs"] - c0["pairs"]), 6),
@@ -455,14 +460,14 @@ def leg_scan_topk(args, torch, lib, _lib, idx, X, Q, n):
             "through_tensor_path": bool(c1["tc"] - c0["tc"] == reps),
             "exact_kernels_same_sample": {"queries": ns, "seconds": round(t_exact, 4), "pairs_per_s": round(ns * n / t_exact, 0)},
             "parity": {"queries": ns, "identical_to_exact_kernels_labels_order_bits": same},
-            "timing": "host wall clock around the C-ABI call (host buffers), median of 3"}
+            "timing": f"host wall clock around the C-ABI call (host buffers), median of {reps}"}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # leg: BASELINE configs[1] (dims 128, N 100K, L2, m 16) on one GPU
 # ---------------------------------------------------------------------------------------------------------------------
 def leg_configs1(args, torch, pg, lib, _lib, local):
-    dims, n, m, efc, efs, B, K, W = 128, 100_000, 16, 200, 64, 32768, 10, 3
+    dims, n, m, efc, efs, B, K, W = 128, 100_000, 16, 200, 64, 32768, args.steps, 3
     g = torch.Generator(device="cuda"); g.manual_seed(99)
     centres = torch.randn((max(4, int(round(n ** 0.5))), dims), generator=g, device="cuda")
     X, Q = gen_points_raw(torch, n, 1234, centres), gen_points_raw(torch, B * (K + W), 5678, centres)
@@ -513,10 +518,8 @@ def leg_configs1(args, torch, pg, lib, _lib, local):
             "value": round(B / (ms * 1e-3), 1), "unit": "queries/s", "ms_per_step": round(ms, 3), "steps": K, "warmup": W, "recall_at_10": round(recall, 4),
             "roofline": {"bound": "instruction issue / hop latency (working set L2-resident)", "achieved": round(alg / (ms * 1e-3) / 1e9, 1), "unit": "GB/s", "algorithmic_bytes_per_launch": alg,
                          "hbm_peak": hbm, "frac_of_hbm_peak": round(alg / (ms * 1e-3) / 1e9 / hbm, 4),
-                         "note": "working set 51 MB vectors + 13 MB links < 126 MB L2: the HBM roof is NOT the binding one here (ncu: DRAM 12 % of peak). "
-                                 "The kernel is bound by instruction issue and the dependent hop chain: 64 % of the issue slots busy with 30 warps per SM, "
-                                 "about 1400 warp instructions of queue / visited / prefetch bookkeeping per hop around 7.5 rows x 512 B of scoring "
-                                 "(profiles/r2_configs1_metrics.csv, profiles/README.md)",
+                         "note": "working set 51 MB vectors + 13 MB links, about the size of the 50 MB L2: mostly L2 hits, so the HBM roof "
+                                 "is not the binding one; the dependent hop chain and the queue / visited bookkeeping per hop are (not profiled on H100)",
                          "per_query": {"dist_evals": float(st[:, 0].mean()), "expansions": float(st[:, 1].mean())}},
             "cpu_baseline": cpu, "parity": par}
 
@@ -529,7 +532,7 @@ def leg_sharded(args, torch, dist, pg, lib, _lib, rank, world, local):
     dims, m, efc, efs = 1536, 32, 200, 64
     rows = int(os.environ.get("PGEMB_BENCH_SHARD_ROWS", 1_250_000))
     B = int(os.environ.get("PGEMB_BENCH_SHARD_BATCH", 16384))
-    K, W = min(args.steps, 10), 2
+    K, W = args.steps, 2
     n_total = rows * world
     lo, hi = sharded.shard_bounds(n_total, world)[rank]
     g = torch.Generator(device="cuda"); g.manual_seed(99)
@@ -628,7 +631,7 @@ def leg_configs4(args, torch, dist, pg, lib, _lib, rank, world, local):
     from pg_embedding_b200 import sharded
     dims, k, nq = 768, 10, 1024
     rows = int(os.environ.get("PGEMB_BENCH_C4_ROWS", 12_500_000))
-    K, W = min(args.steps, 5), 2
+    K, W = args.steps, 2
     n_total = rows * world
     lo, hi = sharded.shard_bounds(n_total, world)[rank]
     g = torch.Generator(device="cuda"); g.manual_seed(99)
@@ -716,10 +719,7 @@ def leg_configs4(args, torch, dist, pg, lib, _lib, rank, world, local):
     idx.close()
     del Q
     torch.cuda.empty_cache()
-    try:
-        bf16 = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"])
-    except Exception:
-        bf16 = 1590.0
+    peak_tf32, peak_src = peak_tf32_tflops()
     hbm, _ = measured_peak_gbs()
     t = ms * 1e-3
     flops_gpu = 2.0 * nq * rows * dims
@@ -728,8 +728,8 @@ def leg_configs4(args, torch, dist, pg, lib, _lib, rank, world, local):
                         f"every rank scans its id range on the tensor-core path (K6), per-shard top-k exchanged and merged (K5); no graph",
             "value": round(nq / t, 1), "unit": "queries/s", "ms_per_step": round(ms, 3), "steps": K, "warmup": W, "scaling": "weak (shard size fixed, table grows with N)",
             "pairs_per_s": round(nq * n_total / t, 0),
-            "tensor": {"bound": "tensor", "achieved_per_gpu": round(flops_gpu / t / 1e12, 1), "peak": round(bf16 / 2.0, 1), "unit": "TFLOP/s",
-                       "frac": round(flops_gpu / t / 1e12 / (bf16 / 2.0), 4), "peak_source": "MEASURED_PEAKS.json bf16_tflops / 2 (TF32 runs at half the bf16 rate)"},
+            "tensor": {"bound": "tensor", "achieved_per_gpu": round(flops_gpu / t / 1e12, 1), "peak": round(peak_tf32, 1), "unit": "TFLOP/s",
+                       "frac": round(flops_gpu / t / 1e12 / peak_tf32, 4), "peak_source": peak_src},
             "hbm_bound_one_table_pass_per_query_tile_s": round(qtiles * rows * dims * 4 / (hbm * 1e9), 5),
             "x_of_that_bound": round(t / (qtiles * rows * dims * 4 / (hbm * 1e9)), 2),
             "rescored_fraction": round((c1["rescored"] - c0["rescored"]) / max(1, c1["pairs"] - c0["pairs"]), 8),

@@ -1,5 +1,5 @@
 /*
- * pgemb_b200.h -- C ABI of the B200-native HNSW candidate-scoring path for pg_embedding.
+ * pgemb_b200.h -- C ABI of the H100-native (sm_90a) HNSW candidate-scoring path for pg_embedding.
  *
  * Two groups of entry points:
  *
@@ -192,7 +192,7 @@ pgemb_status pgemb_dist_gather(pgemb_index *idx, size_t nq, const coord_t *queri
 pgemb_status pgemb_scan_topk(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out,
                              dist_t *dists_out, int32_t *n_out);
 /* How pgemb_scan_topk gets there (DESIGN.md section 6, K6): for L2 and cosine the table is first FILTERED by one dense
- * contraction on the tensor cores (tcgen05.mma kind::tf32, TMA tensor maps, TMEM accumulators; csrc/scan_umma_kernel.cuh) --
+ * contraction on the tensor cores (wgmma tf32, TMA tensor maps, register accumulators; csrc/scan_umma_kernel.cuh) --
  * a row is dropped only if a rigorous lower bound of its distance exceeds the query's current k-th best exact distance --
  * and the survivors are re-scored with the reference-exact arithmetic, so labels, order and distance bits are those of
  * the exact kernels.  Manhattan (no bilinear form) and small tables use the exact tiled kernel throughout.
@@ -206,7 +206,7 @@ void pgemb_scan_counters(uint64_t out[6]);
 pgemb_status pgemb_scan_topk_device(pgemb_index *idx, size_t nq, const coord_t *d_queries, size_t k, label_t *d_labels_out,
                                     dist_t *d_dists_out, int32_t *d_n_out, void *stream);
 /* Test entry: the raw tensor-core products S[q][j] = q . row(r0 + j) (TF32 operands, fp32 accumulate) of the K6 kernel,
- * out[nq * nr], host pointers -- lets a test check descriptors / swizzle / TMEM read-back against a float64 product. */
+ * out[nq * nr], host pointers -- lets a test check descriptors / swizzle / accumulator layout against a float64 product. */
 pgemb_status pgemb_debug_umma_product(pgemb_index *idx, size_t nq, const coord_t *queries, size_t r0, size_t nr, float *out);
 
 /* ---- index-scan iteration: the reference's beginscan / gettuple / endscan trio -- embedding.c:249-387; SURVEY.md 8(f2) ----

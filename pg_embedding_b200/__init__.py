@@ -1,4 +1,4 @@
-"""pg_embedding_b200 -- B200-native (sm_100a) HNSW candidate-scoring path for pg_embedding.
+"""pg_embedding_b200 -- H100-native (sm_90a) HNSW candidate-scoring path for pg_embedding.
 
 The product is the C-ABI shared library ``libpgemb_b200.so`` (include/pgemb_b200.h); this package holds
 its CUDA sources (csrc/), the build script and a thin host-side mirror of the reference's interface for

@@ -1,8 +1,9 @@
-"""Build libpgemb_b200.so (the C-ABI shared library: CUDA kernels for sm_100a + host code) in-tree.
+"""Build libpgemb_b200.so (the C-ABI shared library: CUDA kernels for sm_90a + host code) in-tree.
 
     python -m pg_embedding_b200.build          # or: python pg_embedding_b200/build.py
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with the tree.
+nvcc cross-compiles without a GPU.  The build products are git-ignored and stay in the package directory, so the
+package is importable from the source tree.
 """
 from __future__ import annotations
 
@@ -44,7 +45,7 @@ def needs_build(out: str = OUT) -> bool:
 def _cmd(out: str, verbose: bool) -> list:
     return [
         nvcc_path(), "-shared", "-Xcompiler", "-fPIC", "-std=c++17", "-O3", "-lineinfo",
-        "-gencode", "arch=compute_100a,code=sm_100a",
+        "-gencode", "arch=compute_90a,code=sm_90a",
         "-fmad=false",  # exact kernels use explicit _rn intrinsics; never contract anything else either
         "-Xptxas", "-v" if verbose else "-warn-spills",
         "-I", os.path.join(HERE, "..", "include"),

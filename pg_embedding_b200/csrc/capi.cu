@@ -47,7 +47,7 @@ static pgemb_status fail(pgemb_status st, const std::string &msg)
 	} while (0)
 
 extern "C" const char *pgemb_last_error(void) { return g_last_error.c_str(); }
-extern "C" const char *pgemb_version(void) { return "pg_embedding_b200 0.2 (sm_100a)"; }
+extern "C" const char *pgemb_version(void) { return "pg_embedding_b200 0.2 (sm_90a)"; }
 extern "C" uint64_t	   pgemb_launch_count(void) { return g_launches.load(); }
 
 extern "C" int pgemb_device_count(void)
@@ -1214,13 +1214,13 @@ static pgemb_status launch_scan_filter(pgemb_index *idx, int metric, const float
 	const uint32_t grid = tiles < (uint32_t) idx->sm_count ? tiles : (uint32_t) idx->sm_count;
 	if (metric == DIST_L2)
 	{
-		CU_TRY(cudaFuncSetAttribute(scan_filter_umma_kernel<M_L2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kUmmaSmem));
-		scan_filter_umma_kernel<M_L2><<<grid, kUmmaThreads, kUmmaSmem, s>>>(tq, tv, p);
+		CU_TRY(cudaFuncSetAttribute(scan_filter_wgmma_kernel<M_L2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kUmmaSmem));
+		scan_filter_wgmma_kernel<M_L2><<<grid, kUmmaThreads, kUmmaSmem, s>>>(tq, tv, p);
 	}
 	else
 	{
-		CU_TRY(cudaFuncSetAttribute(scan_filter_umma_kernel<M_COS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kUmmaSmem));
-		scan_filter_umma_kernel<M_COS><<<grid, kUmmaThreads, kUmmaSmem, s>>>(tq, tv, p);
+		CU_TRY(cudaFuncSetAttribute(scan_filter_wgmma_kernel<M_COS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kUmmaSmem));
+		scan_filter_wgmma_kernel<M_COS><<<grid, kUmmaThreads, kUmmaSmem, s>>>(tq, tv, p);
 	}
 	g_launches++;
 	CU_TRY(cudaGetLastError());
@@ -1510,7 +1510,7 @@ static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *q
 }
 
 // Debug / test entry: the raw tensor-core products S[q][j] = q . row(r0 + j) of the K6 kernel (TF32 operands, fp32
-// accumulate), so that a test can check the UMMA descriptors, the swizzled TMA tiles and the TMEM read-back against a
+// accumulate), so that a test can check the wgmma descriptors, the swizzled TMA tiles and the accumulator layout against a
 // float64 product directly.  Host pointers; out[nq * nr].
 extern "C" pgemb_status pgemb_debug_umma_product(pgemb_index *idx, size_t nq, const coord_t *queries, size_t r0, size_t nr, float *out)
 {

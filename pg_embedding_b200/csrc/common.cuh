@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for the B200 (sm_100a) HNSW candidate-scoring path.
+// common.cuh -- shared device/host helpers for the H100 (sm_90a) HNSW candidate-scoring path.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -63,7 +63,7 @@ __device__ __forceinline__ uint64_t key_order(uint64_t k) { return k >> 1; }	// 
 
 #ifndef PGEMB_HOST_EMULATION  // tests/emu supplies host versions of the PTX wrappers below
 // ---------------------------------------------------------------------------------------------
-// Blackwell async-copy plumbing: mbarrier + 1-D bulk TMA (cp.async.bulk -> SASS UBLKCP).
+// Hopper async-copy plumbing: mbarrier + 1-D bulk TMA (cp.async.bulk -> SASS UBLKCP).
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t) __cvta_generic_to_shared(p); }
 
@@ -120,7 +120,7 @@ __device__ __forceinline__ void tma_load_1d(void *dst_smem, const void *src_gmem
 
 // NOTE (kept from the LDGSTS gather experiments, rounds 1-2: measured slower than the bulk copies at every row size and
 // removed, profiles/README.md): `cp.async.cg.shared.global.L2::cache_hint` miscompiles with
-// ptxas 12.9 for sm_100a -- it emits `LDGSTS [R+UR0], desc[UR1]` whose uniform registers are never written and the
+// ptxas 12.9 for sm_100a (the architecture of those experiments) -- it emits `LDGSTS [R+UR0], desc[UR1]` whose uniform registers are never written and the
 // instruction traps ("illegal instruction", pinpointed with compute-sanitizer).  Bulk TMA takes the same policy fine.
 
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }

@@ -1,17 +1,16 @@
 // scan_umma_kernel.cuh -- K6: the brute-force operator path (`ORDER BY val <op> q LIMIT k` without the index,
 // embedding.c:1022-1062 + embedding--0.3.6.sql:20-44; SURVEY.md 8(f3), section 2 "K6") as ONE dense contraction on the
-// 5th-generation tensor cores of sm_100a.  This is the only place of the extension where a batched-query x row-block
-// contraction is genuinely dense, so it is the only kernel here that uses tcgen05.mma / TMEM / TMA tensor maps.
+// tensor cores of sm_90a.  This is the only place of the extension where a batched-query x row-block contraction is
+// genuinely dense, so it is the only kernel here that uses wgmma / TMA tensor maps.
 //
-//     S[q][r] = sum_d Q[q][d] * V[r][d]          kind::tf32, fp32 accumulate in TMEM, operands K-major in shared memory
+//     S[q][r] = sum_d Q[q][d] * V[r][d]          tf32 wgmma, fp32 accumulate in registers, operands K-major in shared memory
 //
 // A tensor-core product cannot give the reference's bits (TF32 keeps 10 mantissa bits; the reference's summation order is
 // fixed, DESIGN.md section 4), so S is used only to DISCARD rows, never to rank them:
 //
-//   scan_filter_umma_kernel   persistent, warp-specialised: warp 0 = TMA producer (cp.async.bulk.tensor.2d, 128-byte swizzle,
-//                             4-stage mbarrier ring), warp 1 = MMA issuer (one elected thread, tcgen05.mma cta_group::1
-//                             M128 x N256 x K8, two 256-column accumulator stages in TMEM), warps 2-5 = epilogue
-//                             (tcgen05.ld 32x32b: one thread = one query = one TMEM lane).  The epilogue never writes S:
+//   scan_filter_wgmma_kernel  persistent, warp-specialised: warpgroup 0 = TMA producer (one thread, cp.async.bulk.tensor.2d,
+//                             128-byte swizzle, 4-stage mbarrier ring), warpgroups 1-2 = consumers (wgmma m64n256k8 tf32,
+//                             64 queries x 256 rows each, then the filter on the accumulator registers).  S is never written:
 //                             a (query,row) pair survives only if a RIGOROUS lower bound of its distance -- from S, the
 //                             exact squared norms and the TF32 error bound |S - q.v| <= rel |q||v| -- does not exceed the
 //                             query's current k-th best exact distance; survivors go to a per-query candidate list.
@@ -22,7 +21,7 @@
 // The host (capi.cu, scan_topk_impl) walks the table in geometrically growing chunks (256, 512, 1K, ... rows): the first
 // chunk establishes the threshold, every later chunk is filtered with the exact threshold of everything before it, so
 // ~k ln(N/k) + (rows inside the error band) candidates per query are re-scored in total.  Result = the exact path's: same
-// labels, same order, bit-identical distances (tests/test_gpu_parity.py::test_scan_umma_*).  Every re-scored candidate
+// labels, same order, bit-identical distances (tests/test_gpu_scan_umma.py).  Every re-scored candidate
 // also CHECKS the error bound against its exact distance (tripwire -> the host repeats the scan on the exact kernels).
 // A query whose candidate list overflows is re-scored against the whole chunk (exact, slow, still correct).
 // Manhattan has no bilinear form and stays on the exact tiled kernel.
@@ -37,11 +36,11 @@
 
 namespace pgemb {
 
-constexpr uint32_t kUmmaTQ = 128;	  // queries per tile = UMMA M = TMEM lanes
-constexpr uint32_t kUmmaTR = 256;	  // rows per tile    = UMMA N = TMEM columns of one accumulator stage
+constexpr uint32_t kUmmaTQ = 128;	  // queries per tile = two wgmma M = 64 halves
+constexpr uint32_t kUmmaTR = 256;	  // rows per tile    = wgmma N
 constexpr uint32_t kUmmaBK = 32;	  // floats per k-block = one 128-byte swizzle atom
 constexpr uint32_t kUmmaStages = 4;	  // shared-memory ring depth
-constexpr uint32_t kUmmaThreads = 192;
+constexpr uint32_t kUmmaThreads = 384;  // three warpgroups: producer + two consumers
 constexpr uint32_t kUmmaABytes = kUmmaTQ * kUmmaBK * 4;	 // 16 KB
 constexpr uint32_t kUmmaBBytes = kUmmaTR * kUmmaBK * 4;	 // 32 KB
 constexpr uint32_t kUmmaStageBytes = kUmmaABytes + kUmmaBBytes;
@@ -131,7 +130,7 @@ struct ScanFilterParams
 
 #ifndef PGEMB_HOST_EMULATION
 // ---------------------------------------------------------------------------------------------------------------------
-// PTX wrappers (tcgen05 / TMEM / 2-D TMA).  SASS: UTCHMMA-family (UTC*MMA), LDTM, UTMALDG, UTCBAR.
+// PTX wrappers (wgmma / 2-D TMA).  SASS: HGMMA, UTMALDG, SYNCS (mbarrier).
 // ---------------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const CUtensorMap *tmap, uint32_t bar_smem, int32_t c0, int32_t c1)
 {
@@ -141,35 +140,38 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const CUtensorMap
 }
 __device__ __forceinline__ void tmap_prefetch(const CUtensorMap *tmap) { asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void tc05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc05_commit(uint64_t *bar)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulators are written asynchronously: tie every register to this point so that no read is scheduled above the wait
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[128])
 {
-	asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+#pragma unroll
+	for (uint32_t i = 0; i < 128; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[tmem] (+)= A[smem] * B[smem], single-thread issue
-__device__ __forceinline__ void tc05_mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate)
+
+// D[64 x 256] (+)= A[64 x 8] * B[256 x 8]^T, tf32 operands from shared memory (both K-major), fp32 accumulators in registers
+#define PGEMB_D4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define PGEMB_D16(i) PGEMB_D4(i), PGEMB_D4(i + 4), PGEMB_D4(i + 8), PGEMB_D4(i + 12)
+__device__ __forceinline__ void wgmma_m64n256k8_tf32(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate)
 {
 	asm volatile(
 		"{\n\t.reg .pred p;\n\t"
-		"setp.ne.b32 p, %4, 0;\n\t"
-		"tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-		::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+		"setp.ne.b32 p, %130, 0;\n\t"
+		"wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+		"%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, "
+		"%27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, "
+		"%52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, "
+		"%77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, "
+		"%102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, "
+		"%123, %124, %125, %126, %127}, %128, %129, p, 1, 1;\n\t}"
+		: PGEMB_D16(0), PGEMB_D16(16), PGEMB_D16(32), PGEMB_D16(48), PGEMB_D16(64), PGEMB_D16(80), PGEMB_D16(96), PGEMB_D16(112)
+		: "l"(a_desc), "l"(b_desc), "r"(accumulate)
 		: "memory");
 }
-__device__ __forceinline__ void tc05_ld32(uint32_t taddr, uint32_t (&v)[32])
-{
-	asm volatile(
-		"tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-		"%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-		: "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-		  "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-		  "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]),
-		  "=r"(v[31])
-		: "r"(taddr)
-		: "memory");
-}
-__device__ __forceinline__ void tc05_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+#undef PGEMB_D16
+#undef PGEMB_D4
 // mbarrier wait that cannot hang the GPU: a pipeline bug (wrong byte count, wrong parity) would otherwise spin forever.  Every
 // legitimate wait in this kernel is microseconds; after ~2^24 polls (seconds) the kernel traps and the launch fails loudly.
 __device__ __forceinline__ void umma_wait(uint64_t *bar, uint32_t parity)
@@ -179,25 +181,25 @@ __device__ __forceinline__ void umma_wait(uint64_t *bar, uint32_t parity)
 	__trap();
 }
 
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): K-major tile of 128-byte rows written by TMA with
-// CU_TENSOR_MAP_SWIZZLE_128B.  start address >> 4 in [0,14); LBO (ignored for swizzled K-major) = 1 in [16,30); SBO = 1024 B
-// (8 rows x 128 B) >> 4 in [32,46); version 1 (sm_100) in [46,48); layout SWIZZLE_128B (2) in [61,64).
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr)
+// Shared-memory matrix descriptor (sm_90 GMMA): K-major tile of 128-byte rows written by TMA with CU_TENSOR_MAP_SWIZZLE_128B.
+// start address >> 4 in [0,14); LBO (ignored for swizzled K-major) = 1 in [16,30); SBO = 1024 B (8 rows x 128 B) >> 4 in
+// [32,46); layout SWIZZLE_128B (1) in [62,64).
+__device__ __forceinline__ uint64_t wgmma_smem_desc(uint32_t smem_addr)
 {
-	return (uint64_t) ((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t) 1 << 16) | ((uint64_t) (1024u >> 4) << 32) | ((uint64_t) 1 << 46) |
-		   ((uint64_t) 2 << 61);
+	return (uint64_t) ((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t) 1 << 16) | ((uint64_t) (1024u >> 4) << 32) | ((uint64_t) 1 << 62);
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D = F32 (1 @ bit 4), A = B = TF32 (2 @ bits 7, 10), both K-major
-// (bits 15, 16 = 0), N >> 3 @ bit 17, M >> 4 @ bit 24.
-constexpr uint32_t kUmmaIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((kUmmaTR >> 3) << 17) | ((kUmmaTQ >> 4) << 24);
 
 // ---------------------------------------------------------------------------------------------------------------------
 // The filter kernel.  grid = min(tiles, SMs) persistent CTAs; tile t -> (row tile t / n_qtiles, query tile t % n_qtiles):
 // CTAs that run at the same time share row tiles, so the table streams from HBM once and is re-read from L2.
+// Warpgroup 0 is the TMA producer (one thread), warpgroups 1 and 2 each own 64 of the tile's 128 queries: they issue the
+// wgmma chain of the tile (m64n256k8, 4 per k-block, one k-block in flight while the previous ring slot is released) and
+// then filter their accumulators in registers.
+// Accumulator layout (per warpgroup, thread = warp w, lane l): d[4 i + 2 h + b] = S[16 w + l / 4 + 8 h][8 i + 2 (l % 4) + b].
 // ---------------------------------------------------------------------------------------------------------------------
 template <int METRIC>
 __global__ void __launch_bounds__(kUmmaThreads, 1)
-	scan_filter_umma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_v, const ScanFilterParams p)
+	scan_filter_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_v, const ScanFilterParams p)
 {
 	static_assert(METRIC == M_L2 || METRIC == M_COS, "the filter needs a bilinear form");
 	extern __shared__ unsigned char umma_smem_raw[];
@@ -206,10 +208,9 @@ __global__ void __launch_bounds__(kUmmaThreads, 1)
 	unsigned char *ring_p = umma_smem_raw + (ring - raw);
 	float2		  *rc_s = reinterpret_cast<float2 *>(ring_p + kUmmaStages * kUmmaStageBytes);  // [2][kUmmaTR]
 	uint64_t	  *bars = reinterpret_cast<uint64_t *>(ring_p + kUmmaStages * kUmmaStageBytes + 2 * kUmmaTR * 8);
-	uint64_t	  *full = bars, *empty = bars + kUmmaStages, *tfull = bars + 2 * kUmmaStages, *tempty = bars + 2 * kUmmaStages + 2;
-	uint32_t	  *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * kUmmaStages + 4);
+	uint64_t	  *full = bars, *empty = bars + kUmmaStages;
 
-	const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+	const uint32_t wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 	const uint32_t n_tiles = p.n_qtiles * p.n_rtiles;
 
 	if (threadIdx.x == 0)
@@ -217,32 +218,19 @@ __global__ void __launch_bounds__(kUmmaThreads, 1)
 		for (uint32_t s = 0; s < kUmmaStages; s++)
 		{
 			mbar_init(&full[s], 1);
-			mbar_init(&empty[s], 1);
-		}
-		for (uint32_t a = 0; a < 2; a++)
-		{
-			mbar_init(&tfull[a], 1);
-			mbar_init(&tempty[a], 4);  // one arrival per epilogue warp
+			mbar_init(&empty[s], 8);  // one arrival per consumer warp
 		}
 		fence_mbar_init();
 		tmap_prefetch(&tmap_q);
 		tmap_prefetch(&tmap_v);
 	}
-	if (warp == 1)
-	{
-		// all 512 TMEM columns: two accumulator stages of 256 fp32 columns (one CTA per SM, so nobody else allocates)
-		asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-		asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-	}
-	tc05_fence_before();
 	__syncthreads();
-	tc05_fence_after();
-	const uint32_t tmem_base = *tmem_slot;
 
-	if (warp == 0)
+	if (wg == 0)
 	{
 		// ===== TMA producer (one thread) =====
-		if (lane == 0)
+		asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+		if (warp == 0 && lane == 0)
 		{
 			uint32_t it = 0;
 			for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x)
@@ -260,107 +248,112 @@ __global__ void __launch_bounds__(kUmmaThreads, 1)
 				}
 			}
 		}
+		return;
 	}
-	else if (warp == 1)
-	{
-		// ===== MMA issuer (one thread) =====
-		if (lane == 0)
-		{
-			uint32_t it = 0, ti = 0;
-			for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x, ti++)
-			{
-				const uint32_t as = ti & 1u, aph = (ti >> 1) & 1u;
-				umma_wait(&tempty[as], aph ^ 1u);  // the epilogue has drained this accumulator stage
-				tc05_fence_after();
-				const uint32_t d_tmem = tmem_base + as * kUmmaTR;
-				for (uint32_t kb = 0; kb < p.kblocks; kb++, it++)
-				{
-					const uint32_t s = it % kUmmaStages, ph = (it / kUmmaStages) & 1u;
-					umma_wait(&full[s], ph);
-					tc05_fence_after();
-					const uint32_t a_src = ring + s * kUmmaStageBytes, b_src = a_src + kUmmaABytes;
-					const uint64_t a_desc = umma_smem_desc(a_src), b_desc = umma_smem_desc(b_src);
+
+	// ===== consumers: warpgroups 1, 2 =====
+	asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+	const uint32_t cw = warp & 3u;						// warp inside the warpgroup
+	const uint32_t ct = threadIdx.x - 128u;				// 0..255
+	const uint32_t a_off = (wg - 1u) * 64u * 128u;		// this warpgroup's 64 query rows of the A tile
+	const uint32_t quad = lane & 3u;
+	uint32_t	   it = 0, ti = 0;
+	float		   d[128];
 #pragma unroll
-					for (uint32_t j = 0; j < kUmmaBK / 8; j++)	// K = 8 tf32 (32 bytes) per instruction: +2 in the 16-byte address field
-						tc05_mma_tf32(d_tmem, a_desc + 2 * j, b_desc + 2 * j, kUmmaIdesc, (kb | j) != 0u ? 1u : 0u);
-					tc05_commit(&empty[s]);	 // frees the ring slot when these MMAs have read it
-				}
-				tc05_commit(&tfull[as]);  // accumulator complete
-			}
-		}
-	}
-	else
+	for (uint32_t i = 0; i < 128; i++) d[i] = 0.0f;
+	for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x, ti++)
 	{
-		// ===== epilogue: 4 warps, thread = query = TMEM lane =====
-		const uint32_t quarter = warp & 3u;	 // the TMEM lane quarter this warp may access
-		const uint32_t et = threadIdx.x - 64u;  // 0..127
-		uint32_t	   ti = 0;
-		for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x, ti++)
+		const uint32_t rt = t / p.n_qtiles, qt = t % p.n_qtiles;
+		const uint32_t row_rel0 = rt * kUmmaTR;					 // first row of the tile, relative to r0
+		const uint32_t valid = min(kUmmaTR, p.nr - row_rel0);	 // rows of this tile inside the chunk
+		// row constants of the tile -> shared memory (one row per thread; double-buffered: the barrier below also orders the
+		// other warpgroup's reads of the previous tile before these writes are reused two tiles later)
+		float2 *rc = rc_s + (ti & 1u) * kUmmaTR;
+		rc[ct] = (ct < valid) ? filter_rconst<METRIC>(p.vnorm2[p.r0 + row_rel0 + ct]) : make_float2(0.f, 0.f);
+		asm volatile("bar.sync 1, 256;" ::: "memory");
+
+		// ---- the product: one k-block in flight, the ring slot of the previous one is released as soon as it retires ----
+		for (uint32_t kb = 0; kb < p.kblocks; kb++, it++)
 		{
-			const uint32_t as = ti & 1u, aph = (ti >> 1) & 1u;
-			const uint32_t rt = t / p.n_qtiles, qt = t % p.n_qtiles;
-			const uint32_t row_rel0 = rt * kUmmaTR;								 // first row of the tile, relative to r0
-			const uint32_t valid = min(kUmmaTR, p.nr - row_rel0);				 // rows of this tile inside the chunk
-			const uint32_t q = qt * kUmmaTQ + quarter * 32u + lane;
+			const uint32_t s = it % kUmmaStages, ph = (it / kUmmaStages) & 1u;
+			umma_wait(&full[s], ph);
+			const uint32_t a_src = ring + s * kUmmaStageBytes + a_off, b_src = ring + s * kUmmaStageBytes + kUmmaABytes;
+			const uint64_t a_desc = wgmma_smem_desc(a_src), b_desc = wgmma_smem_desc(b_src);
+			wgmma_fence();
+#pragma unroll
+			for (uint32_t j = 0; j < kUmmaBK / 8; j++)	// K = 8 tf32 (32 bytes) per instruction: +2 in the 16-byte address field
+				wgmma_m64n256k8_tf32(d, a_desc + 2 * j, b_desc + 2 * j, (kb | j) != 0u ? 1u : 0u);
+			wgmma_commit();
+			wgmma_wait<1>();
+			if (kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % kUmmaStages]);
+		}
+		wgmma_wait<0>();
+		wgmma_fence_regs(d);
+		if (lane == 0) mbar_arrive(&empty[(it - 1) % kUmmaStages]);
+
+		// ---- epilogue: thread = two queries (h = 0, 1) x 64 columns ----
+		const uint32_t qrow = qt * kUmmaTQ + (wg - 1u) * 64u + cw * 16u + (lane >> 2);
+#pragma unroll
+		for (uint32_t h = 0; h < 2; h++)
+		{
+			const uint32_t q = qrow + 8u * h;
 			const bool	   q_ok = q < p.nq;
-			const float2   qc = (q_ok && p.dbg_s == nullptr) ? p.qconst[q] : make_float2(0.f, 0.f);
-			// row constants of the tile -> shared memory (2 rows per thread), overlapping the MMAs of this tile
-			float2 *rc = rc_s + as * kUmmaTR;
-			for (uint32_t c = et; c < kUmmaTR; c += 128u) rc[c] = (c < valid) ? filter_rconst<METRIC>(p.vnorm2[p.r0 + row_rel0 + c]) : make_float2(0.f, 0.f);
-			asm volatile("bar.sync 1, 128;" ::: "memory");
-			umma_wait(&tfull[as], aph);
-			tc05_fence_after();
-			const uint32_t taddr = tmem_base + as * kUmmaTR + ((quarter * 32u) << 16);
-			for (uint32_t c0 = 0; c0 < valid; c0 += 32u)
+			if (p.dbg_s != nullptr)
 			{
-				uint32_t v[32];
-				__syncwarp();
-				tc05_ld32(taddr + c0, v);
-				tc05_wait_ld();
-				if (p.dbg_s != nullptr)
+				if (q_ok)
 				{
-					if (q_ok)
-					{
 #pragma unroll
-						for (uint32_t j = 0; j < 32u; j++)
-							if (c0 + j < valid) p.dbg_s[(size_t) q * p.nr + row_rel0 + c0 + j] = __uint_as_float(v[j]);
-					}
+					for (uint32_t i = 0; i < kUmmaTR / 8; i++)
+#pragma unroll
+						for (uint32_t b = 0; b < 2; b++)
+						{
+							const uint32_t c = 8u * i + 2u * quad + b;
+							if (c < valid) p.dbg_s[(size_t) q * p.nr + row_rel0 + c] = d[4 * i + 2 * h + b];
+						}
 				}
-				else if (q_ok)
-				{
-					// survivors of these 32 columns: ONE slot reservation per thread (= per query) and chunk, then the entries
-					uint32_t pass = 0u;
-#pragma unroll
-					for (uint32_t j = 0; j < 32u; j++)
-						if (filter_pass<METRIC>(__uint_as_float(v[j]), qc, rc[c0 + j]) && c0 + j < valid) pass |= 1u << j;
-					if (pass != 0u)
-					{
-						const uint32_t first = atomicAdd(&p.cand_n[q], (uint32_t) __popc(pass));
-#pragma unroll
-						for (uint32_t j = 0; j < 32u; j++)
-							if (pass & (1u << j))
-							{
-								const uint32_t slot = first + (uint32_t) __popc(pass & ((1u << j) - 1u));
-								if (slot < p.cap)
-								{
-									p.cand_rows[(size_t) q * p.cap + slot] = p.r0 + row_rel0 + c0 + j;
-									p.cand_s[(size_t) q * p.cap + slot] = __uint_as_float(v[j]);
-								}
-							}
-					}
-				}
+				continue;
 			}
-			tc05_fence_before();
-			__syncwarp();
-			if (lane == 0) mbar_arrive(&tempty[as]);
+			const float2 qc = q_ok ? p.qconst[q] : make_float2(0.f, 0.f);
+			// survivors: bit 2 i + b of `pass` = column 8 i + 2 (l % 4) + b
+			uint64_t pass = 0;
+#pragma unroll
+			for (uint32_t i = 0; i < kUmmaTR / 8; i++)
+#pragma unroll
+				for (uint32_t b = 0; b < 2; b++)
+				{
+					const uint32_t c = 8u * i + 2u * quad + b;
+					if (q_ok && c < valid && filter_pass<METRIC>(d[4 * i + 2 * h + b], qc, rc[c])) pass |= 1ull << (2 * i + b);
+				}
+			// ONE slot reservation per query and tile: the four lanes of a quad share the query, so their counts are summed
+			const uint32_t cnt = (uint32_t) __popcll(pass);
+			uint32_t	   incl = cnt;
+#pragma unroll
+			for (uint32_t off = 1; off < 4; off <<= 1)
+			{
+				const uint32_t v = __shfl_up_sync(kFull, incl, off, 4);
+				if (quad >= off) incl += v;
+			}
+			const uint32_t total = __shfl_sync(kFull, incl, 3, 4);
+			uint32_t	   first = 0;
+			if (quad == 0 && total != 0u) first = atomicAdd(&p.cand_n[q], total);
+			first = __shfl_sync(kFull, first, 0, 4) + incl - cnt;
+			if (pass != 0ull)
+			{
+#pragma unroll
+				for (uint32_t i = 0; i < kUmmaTR / 8; i++)
+#pragma unroll
+					for (uint32_t b = 0; b < 2; b++)
+						if (pass & (1ull << (2 * i + b)))
+						{
+							const uint32_t slot = first + (uint32_t) __popcll(pass & ((1ull << (2 * i + b)) - 1ull));
+							if (slot < p.cap)
+							{
+								p.cand_rows[(size_t) q * p.cap + slot] = p.r0 + row_rel0 + 8u * i + 2u * quad + b;
+								p.cand_s[(size_t) q * p.cap + slot] = d[4 * i + 2 * h + b];
+							}
+						}
+			}
 		}
-	}
-	tc05_fence_before();
-	__syncthreads();
-	if (warp == 1)
-	{
-		tc05_fence_after();
-		asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
 	}
 }
 #endif	// PGEMB_HOST_EMULATION
@@ -588,7 +581,7 @@ __global__ void scan_qconst_init_kernel(const float *__restrict__ qnorm2, uint32
 }
 
 #ifdef PGEMB_HOST_EMULATION
-// Host stand-in for scan_filter_umma_kernel (tests/emu only): the same predicate on a product whose operands are cut to
+// Host stand-in for scan_filter_wgmma_kernel (tests/emu only): the same predicate on a product whose operands are cut to
 // TF32 (10 mantissa bits, truncation) and, with PGEMB_EMU_GEMM_ERR_PPM = x, pushed by +-x ppm of |q||v|: truncation + push up to
 // 90 % of the assumed bound must still give exact results, 4x the bound must trip the tripwire.  (The truncation alone can use
 // 2 * 2^-10 of the bound -- one-dimensional rows do -- so a test's push has to leave that much room.)

@@ -3,12 +3,12 @@
 // It holds one device index (pgemb_index, the HBM mirror of a relation's graph) per relation key and serves the
 // requests backends publish in shared memory.  Searches that are pending at the same time -- the reference issues
 // hnsw_search one query per call, one call per backend at a time (embedding.c:317,335) -- are gathered per
-// (relation, efSearch) into ONE pgemb_search_batch launch: a single query cannot fill a B200, the concurrent queries
+// (relation, efSearch) into ONE pgemb_search_batch launch: a single query cannot fill an H100, the concurrent queries
 // of many backends can (DESIGN.md section 6).  Everything else (mirror maintenance, hnsw_bind_point, link write-back)
 // is run one request at a time, which is also the reference's rule for writers (embedding.c:627-629: X-lock on page 0).
 //
 // The library that does the work is dlopen()ed (--lib, default: libpgemb_b200.so next to this executable), so the
-// same binary serves the product library on a B200 and, in the CPU test-suite, the host-emulated build of it.
+// same binary serves the product library on the GPU and, in the CPU test-suite, the host-emulated build of it.
 // There is no computation in this file: no CPU fallback exists here either.
 #include <dlfcn.h>
 #include <errno.h>

@@ -78,7 +78,7 @@ def dist_batch(metric, a, b) -> np.ndarray:
 
 
 class HnswIndex:
-    """`CREATE INDEX ... USING hnsw(col) WITH (dims=, m=, efconstruction=, efsearch=)` on a B200."""
+    """`CREATE INDEX ... USING hnsw(col) WITH (dims=, m=, efconstruction=, efsearch=)` on a GPU."""
 
     def __init__(self, dims: int, m: int = DEFAULT_M, efconstruction: int = DEFAULT_EF_CONSTRUCT,
                  efsearch: int = DEFAULT_EF_SEARCH, metric="l2", capacity: int = 1 << 16, device: int = 0):

@@ -24,7 +24,7 @@ int main()
 							sh.link_stride = (maxM + 1 + 3) & ~3u;
 							sh.maxM = maxM;
 							sh.ef = ef;
-							sh.sm_count = 148;
+							sh.sm_count = 132;  // H100 SXM
 							sh.tpr = tpr;
 							SearchTuning tu;
 							SearchConfig c;

@@ -1,7 +1,7 @@
 """pytest configuration: the `gpu` marker and shared fixtures.
 
 `-m "not gpu"`: oracle vs golden vectors / vs the compiled reference, host logic, C-ABI symbol
-checks.  `-m gpu`: parity tests proper, through the C-ABI on a real B200.
+checks.  `-m gpu`: parity tests proper, through the C-ABI on a real H100.
 """
 import os
 import sys
@@ -14,7 +14,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -29,7 +29,7 @@ def pytest_collection_modifyitems(config, items):
         return          # a missing / unloadable extension must FAIL the gpu tests loudly, never skip them
     if have:
         return
-    skip = pytest.mark.skip(reason="no CUDA device (pgemb_device_count() == 0); run with -m gpu on the B200 box")
+    skip = pytest.mark.skip(reason="no CUDA device (pgemb_device_count() == 0); run with -m gpu on an H100")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

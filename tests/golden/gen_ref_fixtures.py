@@ -1,23 +1,30 @@
 #!/usr/bin/env python
-"""Generate golden fixtures from the UNMODIFIED compiled reference (oracle/_ref/libpgemb_ref.so = /root/reference's
-hnswalg.cpp + distfunc.c built in place by oracle/Makefile, on the flat-memory host).  Run here (needs /root/reference):
+"""Generate golden fixtures from the UNMODIFIED compiled reference (oracle/_ref/libpgemb_ref.so = the reference's
+hnswalg.cpp + distfunc.c built in place by oracle/Makefile, on the flat-memory host).  Needs the reference sources:
 
     python tests/golden/gen_ref_fixtures.py
 
 Writes tests/golden/ref_fixtures.npz: seeded inputs, the reference's link lists after a sequential build, its
 hnsw_search results and its hnsw_dist_func outputs (raw fp32 bits).  tests/test_golden_fixtures.py checks the C
-restatement (and, on a GPU, the CUDA path) against this file without needing the reference tree."""
+restatement (and, on a GPU, the CUDA path) against this file without needing the reference tree.
+
+Writes tests/golden/ref_compare.json: the reference's outputs on the seeded inputs of tests/test_oracle_vs_ref.py (SHA-256
+of the raw bytes) and the HnswMetadata field list of its embedding.h (tests/test_abi.py)."""
+import json
 import os
+import re
 import sys
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import oracle  # noqa: E402
+import test_oracle_vs_ref as vs  # noqa: E402
 
 oracle.build("ref")
-assert oracle.available("ref"), "needs /root/reference to build oracle/_ref"
+assert oracle.available("ref"), "needs the reference sources to build oracle/_ref"
 out = {}
 CASES = [  # name, dims, m, efC, n, metric, tie-heavy?
     ("l2_d8", 8, 4, 16, 300, "l2", False),
@@ -52,3 +59,12 @@ for name, dims, m, efc, n, metric, ties in CASES:
     out[f"{name}.dist_bits"] = oracle.dist_many("ref", metric, q[0], x).view(np.uint32)
 np.savez_compressed(os.path.join(os.path.dirname(os.path.abspath(__file__)), "ref_fixtures.npz"), **out)
 print("wrote ref_fixtures.npz with", len(out), "arrays")
+
+cmp = {"dist": {m: vs.distance_outputs(oracle, "ref", m) for m in vs.METRICS},
+       "cosine_parts": vs.digest(np.array([oracle.dist("ref", "cosine", a, b) for a, b in vs.cosine_parts_inputs()], np.float32)),
+       "build_search": {f"{m}.{vs.cfg_id(c)}": vs.build_and_search_outputs(oracle, "ref", m, c) for m in vs.METRICS for c in vs.CONFIGS},
+       "metadata_fields": re.findall(r"^\s*(?:size_t|idx_t|dist_func_t)\s+(\w+);", open(os.path.join(oracle.REF_SRC, "embedding.h")).read(), re.M)}
+with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "ref_compare.json"), "w") as f:
+    json.dump(cmp, f, indent=1, sort_keys=True)
+    f.write("\n")
+print("wrote ref_compare.json")

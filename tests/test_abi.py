@@ -2,6 +2,7 @@
 include/pgemb_b200.h declares, HnswMetadata has the reference's layout, and the product path fails
 loudly (no fallback) when no CUDA device is usable."""
 import ctypes as C
+import json
 import os
 import re
 
@@ -35,10 +36,9 @@ def test_metadata_layout_matches_reference(lib):
     # embedding.h:28-42: 10 size_t + idx_t + enum
     assert C.sizeof(HnswMetadata) == 10 * 8 + 4 + 4
     assert HnswMetadata.enterpoint_node.offset == 80 and HnswMetadata.dist_func.offset == 84
-    ref_h = "/root/reference/embedding.h"
-    if os.path.isfile(ref_h):
-        ref_fields = re.findall(r"^\s*(?:size_t|idx_t|dist_func_t)\s+(\w+);", open(ref_h).read(), re.M)
-        assert ref_fields == [f[0] for f in HnswMetadata._fields_]
+    # the field list of the reference's embedding.h, recorded by tests/golden/gen_ref_fixtures.py
+    ref_fields = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_compare.json")))["metadata_fields"]
+    assert ref_fields == [f[0] for f in HnswMetadata._fields_]
 
 
 def test_meta_init_follows_hnsw_get_index(lib):
@@ -87,11 +87,10 @@ def test_product_does_not_import_oracle():
                     and "libpgemb_ref" not in src, f
 
 
-def test_product_library_is_blackwell_native(lib):
-    """SASS evidence (B200_PROFILING.md "What proves a Blackwell-native kernel"): the traversal gathers rows with the bulk-copy
-    engine (UBLKCP + mbarrier SYNCS), the brute-force scan's dense contraction runs on the 5th-gen tensor cores
-    (tcgen05.mma -> UTC*MMA, TMEM read-back LDTM, 2-D TMA tensor-map loads UTMALDG) -- and nothing is a legacy mma.sync/wgmma
-    path or a library GEMM (no cuBLAS symbol, no HMMA)."""
+def test_product_library_is_hopper_native(lib):
+    """SASS evidence of a Hopper-native library: the traversal gathers rows with the bulk-copy engine (UBLKCP + mbarrier
+    SYNCS), the brute-force scan's dense contraction runs on the sm_90a tensor cores as warpgroup MMAs fed by 2-D TMA
+    tensor-map loads (wgmma -> HGMMA, UTMALDG) -- and nothing is a legacy mma.sync path (HMMA) or a library GEMM (no cuBLAS)."""
     import shutil
     import subprocess
     from pg_embedding_b200 import build
@@ -99,6 +98,7 @@ def test_product_library_is_blackwell_native(lib):
     if not os.path.isfile(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", build.OUT], capture_output=True, text=True).stdout
+    assert "arch = sm_90a" in sass
     ops = {}
     fn = None
     for line in sass.splitlines():
@@ -106,20 +106,20 @@ def test_product_library_is_blackwell_native(lib):
         if m:
             fn = m.group(1)
             continue
-        m = re.search(r"\s(UTC[A-Z0-9]*MMA|LDTM|UTMALDG|UBLKCP|HMMA|HGMMA|UTCBAR)\b", line)
+        m = re.search(r"\s(UTMALDG|UBLKCP|HMMA|HGMMA)\b", line)
         if m and fn:
             ops.setdefault(fn, {}).setdefault(m.group(1), 0)
             ops[fn][m.group(1)] += 1
-    umma = [f for f in ops if "scan_filter_umma_kernel" in f]
+    umma = [f for f in ops if "scan_filter_wgmma_kernel" in f]
     assert len(umma) == 2, umma                                   # L2 and cosine
     for f in umma:
-        assert any(k.startswith("UTC") and k.endswith("MMA") for k in ops[f]), (f, ops[f])
-        assert ops[f].get("LDTM", 0) >= 1 and ops[f].get("UTMALDG", 0) >= 2 and ops[f].get("UTCBAR", 0) >= 2, (f, ops[f])
+        assert ops[f].get("HGMMA", 0) >= 1 and ops[f].get("UTMALDG", 0) >= 2, (f, ops[f])
+    assert [f for f in ops if "HGMMA" in ops[f]] == umma
     search = [f for f in ops if "search_kernel" in f]
     assert len(search) == 11                                      # 3 metrics x 2 modes + the 8-lanes-per-row L2 pair + 3 huge-ef variants
     for f in search:
         assert ops[f].get("UBLKCP", 0) >= 2, (f, ops[f])
-    assert not any("HMMA" in v or "HGMMA" in v for v in ops.values())
+    assert not any("HMMA" in v for v in ops.values())
     needed = subprocess.run(["ldd", build.OUT], capture_output=True, text=True).stdout
     assert "cublas" not in needed.lower()
     assert "cublas" not in open(os.path.join(ROOT, "pg_embedding_b200", "csrc", "capi.cu")).read().lower()
@@ -171,9 +171,9 @@ def test_c_program_links_against_the_library_and_fails_loudly_without_a_device(l
 
 
 def test_product_kernels_are_the_measured_ones(lib):
-    """The kernels of libpgemb_b200.so must be, instruction for instruction, the ones the numbers in profiles/ and DESIGN.md
-    section 9 were measured with (tests/golden/product_sass.json; refresh it with tools/sass_hash.py --write together with the
-    numbers when a kernel changes on purpose).  Only meaningful with the toolchain that recorded the hashes."""
+    """The kernels of libpgemb_b200.so must be, instruction for instruction, the ones the numbers in DESIGN.md section 9 were
+    measured with (tests/golden/product_sass.json; refresh it with tools/sass_hash.py --write together with the numbers when a
+    kernel changes on purpose).  Only meaningful with the toolchain that recorded the hashes."""
     import json
     import shutil
     import subprocess

@@ -1,6 +1,6 @@
 """The WHOLE library on the host: capi.cu (the C ABI: workspaces, staging, build orchestration, error paths) compiled by
 g++ against tests/emu's stand-in CUDA runtime, its kernels run by the SIMT emulator.  The bodies of the GPU parity tests
-(tests/test_gpu_parity.py) are reused on their small configurations, so the same assertions that gate the B200 run
+(tests/test_gpu_parity.py) are reused on their small configurations, so the same assertions that gate the H100 run
 also exercise the host logic here -- bit-exact against the oracle -- without a GPU.
 
 This is test infrastructure, not a fallback: the emulated library is built into a temporary directory by this module's
@@ -275,7 +275,7 @@ def U():
 @pytest.mark.parametrize("metric", ["l2", "cosine"])
 def test_tensor_core_filter_scan(pg, G, U, oracle_mod, metric, monkeypatch):
     """K6 on the host: the filter predicate, the chunk orchestration, candidate lists and the re-scoring kernel run as compiled;
-    only the tcgen05 product itself is replaced by a TF32-truncated host product that is additionally pushed by +-90 % of the
+    only the wgmma product itself is replaced by a TF32-truncated host product that is additionally pushed by +-90 % of the
     error bound the filter assumes (adversarial but legal).  A product 4x outside the bound must trip the tripwire and the exact
     kernels must take over."""
     for case in ((33, 900, 20, 9), (100, 400, 5, 9), (16, 300, 64, 7), (3, 40, 64, 5)):

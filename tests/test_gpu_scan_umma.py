@@ -1,13 +1,13 @@
 """GPU tests of K6, the tensor-core path of the brute-force operator scan (csrc/scan_umma_kernel.cuh; SURVEY.md 8(f3)):
 
-* the raw tcgen05 products (TMA swizzled tiles -> UMMA descriptors -> TMEM -> tcgen05.ld) against a float64 product,
+* the raw wgmma products (TMA swizzled tiles -> wgmma descriptors -> register accumulators) against a float64 product,
   inside the TF32 error bound the filter assumes, over tile-edge shapes;
 * pgemb_scan_topk through the filter == the exact kernels, bit for bit (labels, order, distances), == the oracle's
   distances sorted by (dist,label): ties, duplicates, deleted labels, k > N, ragged dims, several chunks, candidate-list
   overflow, several query tiles.
 
 tests/test_capi_emulated.py reuses the bodies on the emulated library (the filter predicate, the chunk orchestration, the
-re-scoring kernel; the tcgen05 kernel itself only runs here)."""
+re-scoring kernel; the wgmma kernel itself only runs here)."""
 import ctypes as C
 
 import numpy as np

@@ -1,5 +1,5 @@
-"""GPU parity tests of the kernel / host-path VARIANTS that round 1 had written but not measured and round 2 measured
-(profiles/README.md "round 2, first GPU call"), promoted and turned on by default: the paired visited test-and-set and the
+"""GPU parity tests of the kernel / host-path VARIANTS that round 1 had written but not measured and round 2 measured,
+promoted and turned on by default: the paired visited test-and-set and the
 shared-memory visited set of the latency-mode kernel, 8 lanes per long L2 row, the tiled exact scan, the single-stream host
 path for small batches, the batch clamp of the exact parallel build.  Every variant is exercised with its flag forced ON and
 (tests/test_capi_emulated.py::test_flags_off_give_the_same_results, and the A/B tools) OFF; results must equal the oracle's

@@ -60,7 +60,7 @@ def test_layout_invariants(rows):
         assert r["row_smem"] % 128 == (32 if r["metric"] == 0 else 16), what
         assert r["qt_stride"] % 32 == 4, what                                    # every run 16-byte aligned (LDS.128), runs on distinct banks
         # slots the host allocates per-slot workspace for
-        assert r["slots"] == (148 if r["coop"] else 148 * r["warps"]), what
+        assert r["slots"] == (132 if r["coop"] else 132 * r["warps"]), what
     # what does not fit must say so instead of producing a layout
     for r in rows:
         if r["rc"] != 0:

@@ -6,7 +6,7 @@ searches into batched launches.  What must hold: results identical to the oracle
 reference's ownership / failure behaviour at the boundary, and no hang when either side dies.
 
 CPU suite: the sidecar dlopen()s the host-emulated build of the C-ABI library (tests/emu) -- the protocol, batching and
-host logic are what is under test here.  `-m gpu`: the same through the real libpgemb_b200.so on a B200."""
+host logic are what is under test here.  `-m gpu`: the same through the real libpgemb_b200.so on an H100."""
 import json
 import os
 import signal
