@@ -96,11 +96,13 @@ __host__ __device__ __forceinline__ bool filter_pass(float s, float2 qc, float2 
 	if (METRIC == M_COS) return !(s * rc.x < qc.x);
 	return !(s < (qc.x + rc.x) - qc.y * rc.y);
 }
-// the approximate distance (cosine) / squared distance (L2) the product stands for, and its error bound: the tripwire
+// the approximate distance (cosine) / squared distance (L2) the product stands for, and its error bound: the tripwire.
+// |q||v| is taken as sqrt(qn) sqrt(vn): the product qn vn leaves the fp32 range (subnormal below |q||v| = 2^-63, zero below
+// ~2^-75, inf above 2^64) long before the squared norms do, and would drop the rel term from the slack or make it infinite.
 template <int METRIC>
 __host__ __device__ __forceinline__ void filter_approx(float s, float qn, float vn, float rel, float *approx, float *slack)
 {
-	const float scale = sqrtf(qn * vn);
+	const float scale = sqrtf(qn) * sqrtf(vn);
 	if (METRIC == M_COS)
 	{
 		*approx = 1.0f - s / scale;
@@ -605,7 +607,7 @@ inline void scan_filter_emulated(const float *queries, uint32_t q_stride, const 
 			const float	  *a = queries + (size_t) q * q_stride, *b = vectors + (size_t) row * row_f;
 			float		   s = 0.f;
 			for (uint32_t i = 0; i < dim; i++) s += cut(a[i]) * cut(b[i]);
-			if (perturb != 0.0f) s += (((q * 2654435761u + row * 40503u) >> 7) & 1u ? 1.0f : -1.0f) * perturb * sqrtf(qnorm2[q] * p.vnorm2[row]);
+			if (perturb != 0.0f) s += (((q * 2654435761u + row * 40503u) >> 7) & 1u ? 1.0f : -1.0f) * perturb * sqrtf(qnorm2[q]) * sqrtf(p.vnorm2[row]);
 			if (p.dbg_s)
 			{
 				p.dbg_s[(size_t) q * p.nr + j] = s;

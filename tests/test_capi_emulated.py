@@ -312,6 +312,43 @@ def test_tensor_core_filter_scan(pg, G, U, oracle_mod, metric, monkeypatch):
         U.test_scan_umma_default_policy(pg, monkeypatch)
 
 
+@pytest.fixture(scope="module")
+def B():
+    import test_gpu_scan_filter_bound as b     # GPU tests of the filter's error bound and drop decisions: bodies reused below
+    return b
+
+
+def test_tensor_core_filter_integer_product(pg, B):
+    """The product stand-in on integer data equals the float64 product (on the GPU this pins the wgmma addressing; here it
+    checks the harness and the debug entry point's ragged shapes)."""
+    for shape in ((1, 40, 1, 1, 39), (8, 700, 129, 1, 699), (33, 300, 3, 7, 293), (100, 300, 2, 1, 299)):
+        B.check_integer_product(pg, shape)
+
+
+@pytest.mark.parametrize("metric", ["l2", "cosine"])
+def test_tensor_core_filter_scale_sweep(pg, B, oracle_mod, metric, monkeypatch):
+    """The filter's slack scales with the data across the whole range where the norms stay normal fp32: no fallback."""
+    B.check_scale_sweep(pg, oracle_mod, metric, monkeypatch, 24, 600, nq=12)
+
+
+@pytest.mark.parametrize("metric", ["l2", "cosine"])
+def test_tensor_core_filter_drop_edges(pg, B, oracle_mod, metric, monkeypatch):
+    """Near-ties inside the error band with tie-breaks across chunks, a large common offset, zero vectors, and the tripwire
+    on a bound far too small (exactly one fallback)."""
+    B.check_near_ties(pg, oracle_mod, metric, monkeypatch, 24, 1200)
+    B.check_offset_and_zeros(pg, oracle_mod, metric, monkeypatch, 16, 700, nq=12)
+    B.check_tripwire(pg, oracle_mod, metric, monkeypatch, 64, 400, nq=8)
+
+
+@pytest.mark.parametrize("metric", ["l2", "cosine"])
+def test_tensor_core_filter_orchestration(pg, B, oracle_mod, metric, monkeypatch):
+    """k at the shared-memory top-k edge (256 / 257) and at the maximum (4096), more queries than one query group through
+    both entry points, and the chunk-policy knobs with the short-last-chunk merge."""
+    B.check_k_edges(pg, oracle_mod, metric, monkeypatch, (256, 257, 4096), 10000, nq=6)
+    B.check_query_groups(pg, oracle_mod, metric, monkeypatch, 300, dims=8, k=5)
+    B.check_chunk_policy(pg, oracle_mod, metric, monkeypatch, 1044, nq=8)
+
+
 def test_prototype_l2_eight_lanes(pg_proto, G, oracle_mod, monkeypatch):
     pg = pg_proto
     monkeypatch.setenv("PGEMB_L2_TPR8", "1")

@@ -37,7 +37,7 @@ if __name__ == "__main__":
     from pg_embedding_b200 import build
     h = sass_hashes(build.build())
     if "--write" in sys.argv:
-        json.dump({"_comment": "SASS hashes of the kernels of libpgemb_b200.so that the numbers in profiles/ and DESIGN.md section 9 were measured with "
+        json.dump({"_comment": "SASS hashes of the kernels of libpgemb_b200.so that the numbers in DESIGN.md section 9 were measured with "
                                "(tools/sass_hash.py --write)", "nvcc": subprocess.run(["nvcc", "--version"], capture_output=True, text=True).stdout.strip().splitlines()[-2],
                    "kernels": h}, open(os.path.join(ROOT, "tests", "golden", "product_sass.json"), "w"), indent=1, sort_keys=True)
     print(json.dumps(h, indent=1, sort_keys=True))
