@@ -13,7 +13,8 @@
  *   (2) the mirror-maintenance calls the glue in embedding.c makes (INTEGRATION.md): attach a relation, ship page
  *       records, read modified link lists back, mark labels deleted, truncate, drop.
  *
- * Concurrent hnsw_search calls of different backends are gathered by the sidecar into one batched traversal launch.
+ * Concurrent hnsw_search calls of different backends are gathered by the sidecar into one batched traversal launch, and
+ * concurrent index-less scans (pgemb_client_scan_topk) into one batched brute-force scan.
  * All functions returning int return 0 on success and a pgemb_status (include/pgemb_b200.h) otherwise;
  * pgemb_client_last_error() describes the last failure of the calling thread.
  */
@@ -70,6 +71,20 @@ int pgemb_client_drop(PgembClientIndex *h);
 int pgemb_client_build(PgembClientIndex *h, size_t first, size_t n, size_t batch_max, int exact, double *seconds_out);
 /* Sidecar counters: search launches, queries served, largest batch (how well concurrent callers were batched). */
 int pgemb_client_stats(uint64_t *n_batches, uint64_t *n_searches, uint64_t *max_batch);
+
+/* The index-less plan: what `SELECT ... ORDER BY val <op> q LIMIT k` returns with the index not used (one hnsw_dist_func per
+ * row, embedding.c:1022-1062, then the executor's sort; the seq-scan block of test/expected/knn.out:63-91), for ONE query over
+ * every row of relation h->rel_key's mirror.  It is pgemb_scan_topk (include/pgemb_b200.h) run by the sidecar:
+ *   labels_out[k]  results ascending by (dist, label); labels with DELETED_FLAG are skipped
+ *   dists_out[k]   optional (NULL): the matching distances, bit-identical to hnsw_dist_func's
+ *   *n_out         number of results (< k when the relation has fewer live rows)
+ * 1 <= k <= min(4096, the sidecar's --max-ef), else PGEMB_ERR_ARG before anything is sent.  Like hnsw_search it goes to this
+ * process's replica and honours the interrupt check and the dead-sidecar bound.  The scans that backends have pending at
+ * the same time for the same (relation, k) are served by one pgemb_scan_topk call: one pass over the table for all of them. */
+int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, label_t *labels_out, dist_t *dists_out, size_t *n_out);
+/* Sidecar scan counters, summed over replicas (largest batch: the maximum): pgemb_scan_topk calls, scans served, largest
+ * batch.  Scans are not counted by pgemb_client_stats. */
+int pgemb_client_scan_stats(uint64_t *n_calls, uint64_t *n_scans, uint64_t *max_batch);
 /* Ask the sidecar to exit (tests, controlled restarts). */
 int pgemb_client_shutdown_server(void);
 

@@ -75,6 +75,10 @@ static double now_s(void)
 static PgembIpcSlot *slot_at(const Conn *c, uint32_t i) { return (PgembIpcSlot *) (c->base + c->hdr->slots_off + (size_t) i * c->hdr->slot_stride); }
 static float		*slot_vec(PgembIpcSlot *s) { return (float *) ((unsigned char *) s + pgemb_ipc_payload_vec_off()); }
 static label_t		*slot_labels(const Conn *c, PgembIpcSlot *s) { return (label_t *) ((unsigned char *) s + pgemb_ipc_payload_labels_off(c->hdr->max_dim)); }
+static dist_t		*slot_dists(const Conn *c, PgembIpcSlot *s)
+{
+	return (dist_t *) ((unsigned char *) s + pgemb_ipc_payload_dists_off(c->hdr->max_dim, c->hdr->max_ef));
+}
 
 static int server_alive(const Conn *c)
 {
@@ -493,6 +497,72 @@ int pgemb_client_stats(uint64_t *n_batches, uint64_t *n_searches, uint64_t *max_
 	if (n_searches) *n_searches = s;
 	if (max_batch) *max_batch = m;
 	return PGEMB_OK;
+}
+
+int pgemb_client_scan_stats(uint64_t *n_calls, uint64_t *n_scans, uint64_t *max_batch)
+{
+	const int rc = ensure_connected();
+	if (rc) return rc;
+	uint64_t c = 0, s = 0, m = 0;
+	for (int i = 0; i < g_nconn; i++)
+	{
+		c += __atomic_load_n(&g_conn[i].hdr->n_scan_calls, __ATOMIC_RELAXED);
+		s += __atomic_load_n(&g_conn[i].hdr->n_scans, __ATOMIC_RELAXED);
+		const uint64_t mi = __atomic_load_n(&g_conn[i].hdr->max_scan_batch, __ATOMIC_RELAXED);
+		if (mi > m) m = mi;
+	}
+	if (n_calls) *n_calls = c;
+	if (n_scans) *n_scans = s;
+	if (max_batch) *max_batch = m;
+	return PGEMB_OK;
+}
+
+/* ---- the index-less scan (embedding.c:1022-1062 per row + the executor's sort; knn.out:63-91) ------------------------- */
+int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, label_t *labels_out, dist_t *dists_out, size_t *n_out)
+{
+	if (!h || !query || !labels_out || !n_out)
+	{
+		set_err("pgemb_client_scan_topk: null argument");
+		return PGEMB_ERR_ARG;
+	}
+	int rc = ensure_connected();
+	if (rc) return rc;
+	const Conn	*c = search_conn();
+	const size_t kmax = c->hdr->max_ef < 4096 ? c->hdr->max_ef : 4096;
+	if (k < 1 || k > kmax)
+	{
+		set_err("pgemb_client_scan_topk: k = %zu outside 1 .. %zu (min(4096, the sidecar's --max-ef))", k, kmax);
+		return PGEMB_ERR_ARG;
+	}
+	if (h->meta.dim < 1 || h->meta.dim > c->hdr->max_dim)
+	{
+		set_err("pgemb_client_scan_topk: dims outside the sidecar's limits");
+		return PGEMB_ERR_ARG;
+	}
+	PgembIpcSlot *s = claim_slot(c);
+	if (!s) return PGEMB_ERR_STATE;
+	s->op = PGEMB_OP_SCAN;
+	s->index_key = h->rel_key;
+	s->a0 = k;
+	memcpy(slot_vec(s), query, h->meta.dim * sizeof(coord_t));
+	rc = submit_wait(c, s);
+	if (rc == PGEMB_OK)
+	{
+		if (s->n_out >= 0 && (size_t) s->n_out <= k)
+		{
+			const size_t n = (size_t) s->n_out;
+			memcpy(labels_out, slot_labels(c, s), n * sizeof(label_t));
+			if (dists_out) memcpy(dists_out, slot_dists(c, s), n * sizeof(dist_t));
+			*n_out = n;
+		}
+		else
+		{
+			set_err("pgemb_client_scan_topk: the sidecar returned %d results for k = %zu", (int) s->n_out, k);
+			rc = PGEMB_ERR_STATE;
+		}
+	}
+	release_slot(s, rc);
+	return interrupted(rc) ? PGEMB_CLIENT_INTERRUPTED : rc;
 }
 
 int pgemb_client_shutdown_server(void) { return simple_request(1, NULL, PGEMB_OP_SHUTDOWN, 0, 0, 0, 0, NULL, NULL, NULL); }

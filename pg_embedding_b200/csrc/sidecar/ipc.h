@@ -7,7 +7,8 @@
  * so the device index has to live in one GPU-owning process and be keyed by relation.  The reference calls
  * hnsw_search one query at a time (embedding.c:317,335); many backends doing so concurrently is exactly the batch the
  * traversal kernel wants, so the sidecar gathers the requests that are pending at the same time into ONE
- * pgemb_search_batch launch.
+ * pgemb_search_batch launch.  Index-less scans (PGEMB_OP_SCAN) are gathered the same way, per (relation, k), into one
+ * pgemb_scan_topk call.
  *
  * One POSIX shared-memory segment:
  *     IpcHeader | IpcSlot[n_slots] (each followed by its payload) | bulk area
@@ -27,7 +28,7 @@
 #include <stddef.h>
 
 #define PGEMB_IPC_MAGIC 0x424d4750u /* "PGMB" */
-#define PGEMB_IPC_VERSION 1u
+#define PGEMB_IPC_VERSION 2u
 
 enum
 {
@@ -53,7 +54,8 @@ enum
 	PGEMB_OP_SIZE = 11,			  /* -> a0 = size, a1 = capacity */
 	PGEMB_OP_BUILD = 12,		  /* a0 = first, a1 = n, a2 = batch_max, a3 = 1: exact (bit-identical to row-by-row), 0: bulk */
 	PGEMB_OP_DIST = 13,			  /* a0 = dim, a1 = metric, payload: a[dim] b[dim] -> a2 = fp32 bits (hnsw_dist_func) */
-	PGEMB_OP_SHUTDOWN = 14
+	PGEMB_OP_SHUTDOWN = 14,
+	PGEMB_OP_SCAN = 15			  /* a0 = k, payload: query[dim] -> n_out, labels[n_out], dists[n_out] (pgemb_scan_topk for one query) */
 };
 
 typedef struct
@@ -74,6 +76,9 @@ typedef struct
 	uint64_t n_searches;	 /* queries served */
 	uint64_t max_batch;		 /* largest batch so far */
 	uint64_t n_requests;	 /* all requests served */
+	uint64_t n_scan_calls;	 /* pgemb_scan_topk calls (scans are not counted in n_batches / n_searches / max_batch) */
+	uint64_t n_scans;		 /* scan queries served */
+	uint64_t max_scan_batch; /* largest scan batch so far */
 } PgembIpcHeader;
 
 typedef struct
@@ -88,14 +93,15 @@ typedef struct
 	int32_t	 n_out;
 	uint32_t abandoned; /* set by a client that stopped waiting (query cancel): whoever sees DONE afterwards frees the slot */
 	char	 err[164];
-	/* payload follows: float vec[2 * max_dim]; uint64_t labels[max_ef]  (8-byte aligned) */
+	/* payload follows: float vec[2 * max_dim]; uint64_t labels[max_ef]  (8-byte aligned); float dists[max_ef] */
 } PgembIpcSlot;
 
 static inline size_t pgemb_ipc_payload_vec_off(void) { return (sizeof(PgembIpcSlot) + 15u) & ~(size_t) 15u; }
 static inline size_t pgemb_ipc_payload_labels_off(uint32_t max_dim) { return pgemb_ipc_payload_vec_off() + (((size_t) 2 * max_dim * 4 + 15u) & ~(size_t) 15u); }
+static inline size_t pgemb_ipc_payload_dists_off(uint32_t max_dim, uint32_t max_ef) { return pgemb_ipc_payload_labels_off(max_dim) + (size_t) max_ef * 8; }
 static inline size_t pgemb_ipc_slot_stride(uint32_t max_dim, uint32_t max_ef)
 {
-	return (pgemb_ipc_payload_labels_off(max_dim) + (size_t) max_ef * 8 + 63u) & ~(size_t) 63u;
+	return (pgemb_ipc_payload_dists_off(max_dim, max_ef) + (size_t) max_ef * 4 + 63u) & ~(size_t) 63u;
 }
 
 #endif

@@ -4,7 +4,9 @@
 // requests backends publish in shared memory.  Searches that are pending at the same time -- the reference issues
 // hnsw_search one query per call, one call per backend at a time (embedding.c:317,335) -- are gathered per
 // (relation, efSearch) into ONE pgemb_search_batch launch: a single query cannot fill an H100, the concurrent queries
-// of many backends can (DESIGN.md section 6).  Everything else (mirror maintenance, hnsw_bind_point, link write-back)
+// of many backends can (DESIGN.md section 6).  Index-less scans (`ORDER BY val <op> q LIMIT k` without the index) are
+// gathered the same way per (relation, k) into ONE pgemb_scan_topk call: every scan reads the whole table, so sharing
+// that read pays even more there (DESIGN.md section 12).  Everything else (mirror maintenance, hnsw_bind_point, link write-back)
 // is run one request at a time, which is also the reference's rule for writers (embedding.c:627-629: X-lock on page 0).
 //
 // The library that does the work is dlopen()ed (--lib, default: libpgemb_b200.so next to this executable), so the
@@ -52,6 +54,7 @@ struct Api
 	pgemb_status (*truncate)(pgemb_index *);
 	pgemb_status (*reserve)(pgemb_index *, size_t);
 	pgemb_status (*search_batch)(pgemb_index *, size_t, const coord_t *, size_t, label_t *, dist_t *, idx_t *, int32_t *, uint32_t *);
+	pgemb_status (*scan_topk)(pgemb_index *, size_t, const coord_t *, size_t, label_t *, dist_t *, int32_t *);
 	bool (*bind_point)(HnswMetadata *, const coord_t *, idx_t);	 // the reference-shaped hnsw_bind_point
 	pgemb_status (*build_bulk)(pgemb_index *, size_t, size_t, size_t, double *);
 	pgemb_status (*build_exact)(pgemb_index *, size_t, size_t, size_t, double *, uint64_t *);
@@ -79,7 +82,7 @@ bool load_api(const char *path, Api &a)
 		   sym(h, "pgemb_index_capacity", a.index_capacity) && sym(h, "pgemb_index_append_records", a.append_records) &&
 		   sym(h, "pgemb_index_export_records", a.export_records) && sym(h, "pgemb_index_get_links", a.get_links) &&
 		   sym(h, "pgemb_index_set_labels", a.set_labels) && sym(h, "pgemb_index_truncate", a.truncate) && sym(h, "pgemb_index_reserve", a.reserve) && sym(h, "pgemb_search_batch", a.search_batch) &&
-		   sym(h, "hnsw_bind_point", a.bind_point) && sym(h, "pgemb_build_bulk", a.build_bulk) && sym(h, "pgemb_build_exact", a.build_exact) &&
+		   sym(h, "pgemb_scan_topk", a.scan_topk) && sym(h, "hnsw_bind_point", a.bind_point) && sym(h, "pgemb_build_bulk", a.build_bulk) && sym(h, "pgemb_build_exact", a.build_exact) &&
 		   sym(h, "hnsw_dist_func", a.dist_func) && sym(h, "hnsw_init_dist_func", a.init_dist_func);
 }
 
@@ -121,6 +124,7 @@ struct Server
 	// per-batch scratch
 	std::vector<float>	  qbuf;
 	std::vector<label_t>  lbuf;
+	std::vector<float>	  dbuf;
 	std::vector<int32_t>  nbuf;
 
 	PgembIpcSlot *slot(uint32_t i) const { return reinterpret_cast<PgembIpcSlot *>(base + hdr->slots_off + (size_t) i * hdr->slot_stride); }
@@ -128,6 +132,10 @@ struct Server
 	label_t		 *slot_labels(PgembIpcSlot *s) const
 	{
 		return reinterpret_cast<label_t *>(reinterpret_cast<unsigned char *>(s) + pgemb_ipc_payload_labels_off(hdr->max_dim));
+	}
+	float *slot_dists(PgembIpcSlot *s) const
+	{
+		return reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(s) + pgemb_ipc_payload_dists_off(hdr->max_dim, hdr->max_ef));
 	}
 	unsigned char *bulk() const { return base + hdr->bulk_off; }
 
@@ -185,7 +193,7 @@ struct Server
 		return true;
 	}
 
-	// ---- everything except searches: one at a time, in slot order ----------------------------------------------------
+	// ---- everything except searches and scans: one at a time, in slot order ------------------------------------------
 	void run_control(PgembIpcSlot *s)
 	{
 		switch (s->op)
@@ -407,11 +415,54 @@ struct Server
 		}
 	}
 
+	// ---- index-less scans: all requests of one (relation, k) that are pending now -> one pgemb_scan_topk per max_batch ----
+	// Grouped by k, not folded into the largest k of the relation: a query's re-scoring work grows with k (DESIGN.md section 6).
+	void run_scans(std::vector<PgembIpcSlot *> &group)
+	{
+		PgembIpcSlot *s0 = group[0];
+		auto		  it = mirrors.find(s0->index_key);
+		const size_t  k = (size_t) s0->a0;
+		if (it == mirrors.end() || k < 1 || k > std::min<size_t>(4096, hdr->max_ef))
+		{
+			for (PgembIpcSlot *s : group)
+				finish(s, PGEMB_ERR_ARG, it == mirrors.end() ? "no device index attached for this relation key" : "scan: k outside 1 .. min(4096, the sidecar's --max-ef)");
+			return;
+		}
+		Mirror		&m = it->second;
+		const size_t dim = m.host.meta.dim;
+		for (size_t lo = 0; lo < group.size(); lo += max_batch)
+		{
+			const size_t nq = std::min(max_batch, group.size() - lo);
+			qbuf.resize(nq * dim);
+			lbuf.resize(nq * k);
+			dbuf.resize(nq * k);
+			nbuf.assign(nq, 0);
+			for (size_t i = 0; i < nq; i++) memcpy(&qbuf[i * dim], slot_vec(group[lo + i]), dim * sizeof(float));
+			const pgemb_status r = api.scan_topk(m.host.dev, nq, qbuf.data(), k, lbuf.data(), dbuf.data(), nbuf.data());
+			hdr->n_scan_calls += 1;
+			hdr->n_scans += nq;
+			if (nq > hdr->max_scan_batch) hdr->max_scan_batch = nq;
+			for (size_t i = 0; i < nq; i++)
+			{
+				PgembIpcSlot *s = group[lo + i];
+				if (r == PGEMB_OK)
+				{
+					const size_t n = (size_t) (nbuf[i] > 0 ? nbuf[i] : 0);
+					s->n_out = nbuf[i];
+					memcpy(slot_labels(s), &lbuf[i * k], n * sizeof(label_t));
+					memcpy(slot_dists(s), &dbuf[i * k], n * sizeof(float));
+				}
+				finish_api(s, r);
+			}
+		}
+	}
+
 	// one pass over the slots; returns the number of requests served
 	size_t serve_once()
 	{
 		std::vector<PgembIpcSlot *> control;
 		std::map<std::pair<uint64_t, uint32_t>, std::vector<PgembIpcSlot *>> searches;
+		std::map<std::pair<uint64_t, uint64_t>, std::vector<PgembIpcSlot *>> scans;
 		size_t found = 0, nsearch = 0;
 		auto   collect = [&]() {
 			  for (uint32_t i = 0; i < hdr->n_slots; i++)
@@ -425,6 +476,8 @@ struct Server
 					  searches[{s->index_key, s->ef}].push_back(s);
 					  nsearch++;
 				  }
+				  else if (s->op == PGEMB_OP_SCAN)
+					  scans[{s->index_key, s->a0}].push_back(s);  // not part of the searches' linger bookkeeping (nsearch / target / carry)
 				  else
 					  control.push_back(s);
 			  }
@@ -465,6 +518,10 @@ struct Server
 			if (target < 1) target = 1;
 			if (target > hdr->n_slots) target = hdr->n_slots;
 		}
+		// Scans last: a scan sees every write whose request completed before it was submitted, as a search does.  They
+		// never linger: a scan call takes milliseconds, and the next batch queues up by itself while it runs.  A scan and a
+		// search of the same mirror never run at the same time (the index's staging buffers and workspace are shared).
+		for (auto &kv : scans) run_scans(kv.second);
 		return found;
 	}
 

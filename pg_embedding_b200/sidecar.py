@@ -2,8 +2,9 @@
 
 The sidecar is the one GPU-owning process of a forked-backend deployment (DESIGN.md section 12, INTEGRATION.md): it keeps
 the HBM mirror of every hnsw relation and gathers the one-query-per-call `hnsw_search` requests of concurrently running
-backends into batched traversal launches.  This module is what tests/test_sidecar.py and tools/bench_sidecar.py use; it
-contains no computation and no fallback -- without a serving sidecar every call fails.
+backends into batched traversal launches, and their index-less scans into batched brute-force scans.  This module is what
+tests/test_sidecar.py, tests/test_sidecar_scan.py and tools/bench_sidecar.py use; it contains no computation and no
+fallback -- without a serving sidecar every call fails.
 """
 from __future__ import annotations
 
@@ -57,6 +58,8 @@ def client() -> C.CDLL:
     lib.pgemb_client_drop.argtypes = [hp]
     lib.pgemb_client_build.argtypes = [hp, sz, sz, sz, C.c_int, C.POINTER(C.c_double)]
     lib.pgemb_client_stats.argtypes = [C.POINTER(C.c_uint64)] * 3
+    lib.pgemb_client_scan_stats.argtypes = [C.POINTER(C.c_uint64)] * 3
+    lib.pgemb_client_scan_topk.argtypes = [hp, C.POINTER(C.c_float), sz, C.POINTER(C.c_uint64), C.POINTER(C.c_float), C.POINTER(sz)]
     lib.pgemb_client_set_interrupt_check.argtypes = [C.c_void_p]
     lib.hnsw_search.argtypes = [C.POINTER(HnswMetadata), C.POINTER(C.c_float), C.POINTER(sz), C.POINTER(C.POINTER(C.c_uint64))]
     lib.hnsw_search.restype = C.c_bool
@@ -87,6 +90,13 @@ def stats() -> dict:
     a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
     _check(client().pgemb_client_stats(C.byref(a), C.byref(b), C.byref(c)))
     return {"batches": a.value, "searches": b.value, "max_batch": c.value}
+
+
+def scan_stats() -> dict:
+    """The sidecar's scan counters: pgemb_scan_topk calls, scans served, largest scan batch (not part of stats())."""
+    a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
+    _check(client().pgemb_client_scan_stats(C.byref(a), C.byref(b), C.byref(c)))
+    return {"calls": a.value, "scans": b.value, "max_batch": c.value}
 
 
 class RemoteIndex:
@@ -195,6 +205,19 @@ class RemoteIndex:
                 returned += 1
         finally:
             self.h.meta.efSearch = ef0      # the reference's HnswIndex is per scan (embedding.c:254)
+
+    def scan_topk(self, q: np.ndarray, k: int) -> dict:
+        """`ORDER BY val <op> q LIMIT k` without the index (knn.out:63-91) for one query, through the sidecar's batched
+        pgemb_scan_topk.  Returns dict(labels[k], dists[k], n) -- one row of HnswIndex.scan_topk (unused tail: ~0 / inf)."""
+        q = np.ascontiguousarray(q, dtype=np.float32).ravel()
+        if q.size != self.dims:
+            raise ValueError(f"Wrong number of dimensions: {q.size} instead of {self.dims} expected")
+        labels = np.full(max(int(k), 1), np.iinfo(np.uint64).max, np.uint64)
+        dists = np.full(max(int(k), 1), np.inf, np.float32)
+        n = C.c_size_t()
+        _check(client().pgemb_client_scan_topk(C.byref(self.h), q.ctypes.data_as(C.POINTER(C.c_float)), int(k),
+                                               labels.ctypes.data_as(C.POINTER(C.c_uint64)), dists.ctypes.data_as(C.POINTER(C.c_float)), C.byref(n)))
+        return {"labels": labels, "dists": dists, "n": n.value}
 
     def bind_point(self, idx: int, efconstruction: int | None = None) -> None:
         if efconstruction is not None:

@@ -1,11 +1,19 @@
 """Throughput / latency of the reference-shaped hnsw_search (one query per call) when P backend PROCESSES call it at the
-same time through pgemb_sidecar (the forked-backend deployment, DESIGN.md section 12) -- on a B200:
+same time through pgemb_sidecar (the forked-backend deployment, DESIGN.md section 12) -- on an H100:
 
     python tools/bench_sidecar.py [--rows 1000000 --dims 768 --m 32 --metric cosine --backends 1,16,64,128 --seconds 5]
 
 Prints one JSON line per backend count: aggregate queries/s, per-call latency percentiles, and how the sidecar batched
 the calls (launches, mean and largest batch).  The graph is built once in the sidecar (bulk build); parity of the results
 is checked by tests/test_sidecar.py, not here.
+
+    python tools/bench_sidecar.py --op scan --k 10 [--backends 1,16,64,256]
+
+measures the index-less plan instead (`ORDER BY val <op> q LIMIT k` without the index): every backend issues one
+pgemb_client_scan_topk per call on the same table, no graph is built.  One JSON line per backend count (scans/s, latency
+percentiles, pgemb_scan_topk calls, mean and largest batch), then two lines timing pgemb_scan_topk in this process on the
+same table with nq = 1 and nq = 1024, for reference.  Every line names the GPU and its power limit.  Parity:
+tests/test_sidecar_scan.py.
 """
 import argparse
 import ctypes as C
@@ -30,6 +38,8 @@ def backend_main(a):
     q = np.load(a.queries)
     q = np.ascontiguousarray(q[rng.permutation(q.shape[0])], dtype=np.float32)
     lib = sidecar.client()
+    if a.op == "scan":
+        return scan_backend_loop(a, idx, lib, q)
     free = C.CDLL(None).free
     free.argtypes = [C.c_void_p]
     n, res = C.c_size_t(), C.POINTER(C.c_uint64)()
@@ -53,6 +63,65 @@ def backend_main(a):
     np.save(a.out, np.array(lat, np.float64))
 
 
+def scan_backend_loop(a, idx, lib, q):
+    """One backend of --op scan: raw ctypes loop around pgemb_client_scan_topk (no numpy in the timed loop)."""
+    f32p = C.POINTER(C.c_float)
+    labels = (C.c_uint64 * a.k)()
+    dists = (C.c_float * a.k)()
+    n = C.c_size_t()
+    h = C.byref(idx.h)
+    ptrs = [q[i].ctypes.data_as(f32p) for i in range(q.shape[0])]
+    open(a.out + ".ready", "w").close()
+    while not os.path.exists(a.go):
+        time.sleep(0.001)
+    lat = []
+    t_end = time.perf_counter() + a.seconds
+    i = 0
+    while True:
+        t0 = time.perf_counter()
+        if t0 >= t_end:
+            break
+        if lib.pgemb_client_scan_topk(h, ptrs[i % len(ptrs)], a.k, labels, dists, C.byref(n)) != 0:
+            raise RuntimeError(lib.pgemb_client_last_error().decode())
+        lat.append(time.perf_counter() - t0)
+        i += 1
+    np.save(a.out, np.array(lat, np.float64))
+
+
+def gpu_info() -> dict:
+    """The card's name and power limit (read-only nvidia-smi query): part of every figure this tool prints."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"], capture_output=True,
+                             text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, plim = [f.strip() for f in out.split(",")]
+        return {"gpu": name, "power_limit_w": float(plim)}
+    except Exception:
+        return {"gpu": None, "power_limit_w": None}
+
+
+def time_in_process_scan(a, X, Q, info):
+    """pgemb_scan_topk in this process on the sidecar's table (same rows, same metric): nq = 1 and nq = 1024."""
+    import pg_embedding_b200 as pg
+    idx = pg.HnswIndex(a.dims, a.m, a.efc, a.efs, a.metric, capacity=a.rows)
+    step = 1 << 17
+    for lo in range(0, a.rows, step):
+        hi = min(a.rows, lo + step)
+        idx.append(np.ascontiguousarray(X[lo:hi]), np.arange(lo, hi, dtype=np.uint64))
+    for nq, reps in ((1, 200), (1024, 10)):
+        q = np.ascontiguousarray(Q[:nq])
+        idx.scan_topk(q, a.k)                                      # warm-up: module load, buffers of this shape
+        t = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            idx.scan_topk(q, a.k)                                  # host buffers: returns when the scan is done
+            t.append(time.perf_counter() - t0)
+        ms = float(np.median(t)) * 1e3
+        print(json.dumps({"op": "scan", "in_process": True, "nq": nq, "k": a.k, "ms_per_call_median": round(ms, 3),
+                          "scans_per_s": round(nq / (ms * 1e-3), 1), "calls": reps,
+                          "workload": f"dims={a.dims} N={a.rows} {a.metric}, pgemb_scan_topk(nq={nq}) in one process, host buffers", **info}), flush=True)
+    idx.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=1_000_000)
@@ -65,6 +134,8 @@ def main():
     ap.add_argument("--seconds", type=float, default=5.0)
     ap.add_argument("--linger-us", type=int, default=None, help="sidecar's --linger-us (default: the sidecar's own default)")
     ap.add_argument("--lib", default=None, help="C-ABI library the sidecar loads (default: the product library)")
+    ap.add_argument("--op", choices=("search", "scan"), default="search", help="search: hnsw_search per call; scan: pgemb_client_scan_topk per call")
+    ap.add_argument("--k", type=int, default=10, help="LIMIT of --op scan")
     ap.add_argument("--numpy-data", action="store_true", help="iid numpy data instead of bench.py's generator (no torch / CUDA in this process: emulated runs)")
     # internal: backend mode
     ap.add_argument("--backend-id", type=int, default=-1)
@@ -103,18 +174,23 @@ def main():
             rec[:, rs - 8:] = np.arange(lo, hi, dtype=np.uint64).view(np.uint8).reshape(hi - lo, 8)
             idx.append_records(rec)
         t_ship = time.time() - t0
-        t_build = idx.build(0, a.rows, batch_max=4096, exact=False)
-        print(f"# shipped {a.rows} records in {t_ship:.1f}s, bulk build {t_build:.1f}s", file=sys.stderr)
+        if a.op == "search":
+            t_build = idx.build(0, a.rows, batch_max=4096, exact=False)
+            print(f"# shipped {a.rows} records in {t_ship:.1f}s, bulk build {t_build:.1f}s", file=sys.stderr)
+        else:
+            print(f"# shipped {a.rows} records in {t_ship:.1f}s (a scan needs no graph)", file=sys.stderr)
+        info = gpu_info()
         qf = os.path.join(tmp, "q.npy")
         np.save(qf, Q)
         for P in [int(x) for x in a.backends.split(",")]:
             go = os.path.join(tmp, f"go{P}")
-            s0 = sidecar.stats()
+            s0 = sidecar.stats() if a.op == "search" else sidecar.scan_stats()
             procs = []
             for b in range(P):
                 out = os.path.join(tmp, f"lat_{P}_{b}.npy")
                 cmd = [sys.executable, os.path.abspath(__file__), "--backend-id", str(b), "--shm", shm, "--queries", qf, "--out", out, "--go", go,
-                       "--dims", str(a.dims), "--m", str(a.m), "--efc", str(a.efc), "--efs", str(a.efs), "--metric", a.metric, "--seconds", str(a.seconds)]
+                       "--dims", str(a.dims), "--m", str(a.m), "--efc", str(a.efc), "--efs", str(a.efs), "--metric", a.metric, "--seconds", str(a.seconds),
+                       "--op", a.op, "--k", str(a.k)]
                 procs.append((subprocess.Popen(cmd), out))
             while not all(os.path.exists(o + ".ready") or p.poll() is not None for p, o in procs):
                 time.sleep(0.01)
@@ -122,12 +198,23 @@ def main():
             for p, _ in procs:
                 assert p.wait() == 0
             lat = np.concatenate([np.load(o) for _, o in procs])
+            pct = {k: round(float(np.percentile(lat, v)) * 1e3, 3) for k, v in (("p50", 50), ("p90", 90), ("p99", 99))}
+            if a.op == "scan":
+                s1 = sidecar.scan_stats()
+                nc, ns = s1["calls"] - s0["calls"], s1["scans"] - s0["scans"]
+                print(json.dumps({"op": "scan", "backends": P, "k": a.k, "scans_per_s": round(lat.size / a.seconds, 1), "calls": int(lat.size),
+                                  "latency_ms": pct, "scan_topk_calls": nc, "mean_batch": round(ns / max(nc, 1), 2), "max_batch_so_far": s1["max_batch"],
+                                  "workload": f"dims={a.dims} N={a.rows} {a.metric} LIMIT {a.k}, one pgemb_client_scan_topk per call per backend process",
+                                  **info}), flush=True)
+                continue
             s1 = sidecar.stats()
             nb, ns = s1["batches"] - s0["batches"], s1["searches"] - s0["searches"]
             print(json.dumps({"backends": P, "queries_per_s": round(lat.size / a.seconds, 1), "calls": int(lat.size),
-                              "latency_ms": {k: round(float(np.percentile(lat, v)) * 1e3, 3) for k, v in (("p50", 50), ("p90", 90), ("p99", 99))},
+                              "latency_ms": pct,
                               "launches": nb, "mean_batch": round(ns / max(nb, 1), 2), "max_batch_so_far": s1["max_batch"],
                               "workload": f"dims={a.dims} N={a.rows} {a.metric} m={a.m} efS={a.efs}, one query per hnsw_search call per backend process"}))
+        if a.op == "scan":
+            time_in_process_scan(a, X, Q, info)
     finally:
         sidecar.client().pgemb_client_disconnect()
         srv.stop()
