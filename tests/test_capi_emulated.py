@@ -349,6 +349,28 @@ def test_tensor_core_filter_orchestration(pg, B, oracle_mod, metric, monkeypatch
     B.check_chunk_policy(pg, oracle_mod, metric, monkeypatch, 1044, nq=8)
 
 
+@pytest.fixture(scope="module")
+def V():
+    import test_gpu_visited_set as v     # GPU tests of the traversal's visited set: bodies reused below
+    return v
+
+
+def test_visited_set_migration_and_reset(pg, V, oracle_mod, monkeypatch):
+    """The global table migrating to the bitmap in throughput mode (one slot serving every query, some of which migrate and
+    some not; then the bitmap alone), at L2 in latency mode with the paired test-and-set, and the 1024-entry shared-memory
+    table.  L2 only: the visited set does not depend on the metric, and the GPU file runs all three.  The log-overflow cases
+    (> 32 768 visits per query) are left to tests/test_gpu_visited_set.py."""
+    V.check_migration_throughput(pg, oracle_mod, "l2", monkeypatch, 2, warps=1, n=4000)
+    V.check_latency_global_hash(pg, oracle_mod, "l2", monkeypatch, 2, 1, n=4000, nq=6)
+    V.check_latency_small_smem_table(pg, oracle_mod, "l2", monkeypatch, 2, nq=2)
+
+
+def test_visited_set_ties_and_layout_sequence(pg, V, oracle_mod, monkeypatch):
+    """Tie overflow with slot reuse on a hash-mode index, and one index searched under a sequence of visited-set layouts."""
+    V.check_ties(pg, oracle_mod, "l2", monkeypatch, 2, n=600)
+    V.check_layout_sequence(pg, oracle_mod, "l2", monkeypatch, 2, 16, 8, 40, 4000, ef_mig=V.MIG_EF[4000]["l2"], nq=8)
+
+
 def test_prototype_l2_eight_lanes(pg_proto, G, oracle_mod, monkeypatch):
     pg = pg_proto
     monkeypatch.setenv("PGEMB_L2_TPR8", "1")
