@@ -16,6 +16,7 @@
 #include <mutex>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "aux_kernels.cuh"
@@ -45,6 +46,24 @@ static pgemb_status fail(pgemb_status st, const std::string &msg)
 		if (_e != cudaSuccess)                                                                                   \
 			return fail(PGEMB_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));                     \
 	} while (0)
+
+// Runs f(std::integral_constant<int, M_...>{}) for the runtime metric and returns its status: a kernel launched inside takes
+// decltype(m)::value.  with_tc_metric covers only the metrics that have a tensor-core path, so that no M_MAN instance of
+// those kernels is compiled.
+template <typename F> static pgemb_status with_metric(int metric, F &&f)
+{
+	if (metric == DIST_L2) return f(std::integral_constant<int, M_L2>{});
+	if (metric == DIST_COSINE) return f(std::integral_constant<int, M_COS>{});
+	if (metric == DIST_MANHATTAN) return f(std::integral_constant<int, M_MAN>{});
+	return fail(PGEMB_ERR_ARG, "unknown distance function");
+}
+
+template <typename F> static pgemb_status with_tc_metric(int metric, F &&f)
+{
+	if (metric == DIST_L2) return f(std::integral_constant<int, M_L2>{});
+	if (metric == DIST_COSINE) return f(std::integral_constant<int, M_COS>{});
+	return fail(PGEMB_ERR_ARG, "no tensor-core path for this metric");
+}
 
 extern "C" const char *pgemb_last_error(void) { return g_last_error.c_str(); }
 extern "C" const char *pgemb_version(void) { return "pg_embedding_b200 0.2 (sm_90a)"; }
@@ -157,6 +176,7 @@ extern "C" pgemb_status pgemb_index_create(const HnswMetadata *meta, size_t capa
 	if (meta->dim == 0 || meta->dim > 65535) return fail(PGEMB_ERR_ARG, "dims out of range (1..65535; stored as uint16 on pages, embedding.c:494)");
 	if (meta->maxM != meta->M * 2) return fail(PGEMB_ERR_ARG, "maxM must be 2*M (embedding.c:224)");
 	if (meta->maxM > 4096) return fail(PGEMB_ERR_ARG, "maxM > 4096 unsupported");
+	if ((int) meta->dist_func < 0 || (int) meta->dist_func > 2) return fail(PGEMB_ERR_ARG, "unknown distance function");
 	if (capacity == 0 || capacity >= (1ull << 31)) return fail(PGEMB_ERR_ARG, "capacity must be in [1, 2^31)");
 	int ndev = 0;
 	CU_TRY(cudaGetDeviceCount(&ndev));
@@ -253,6 +273,31 @@ static pgemb_status ensure_stage(pgemb_index *idx, size_t bytes)
 	idx->stage_bytes = want;
 	return PGEMB_OK;
 }
+
+// Arrays carved out of one staging buffer, back to back in the order listed, each starting 256-byte aligned.  `bytes` is
+// what the buffer must hold; place() points every array at its part of the buffer.
+struct StageLayout
+{
+	struct Part
+	{
+		template <typename T> Part(T *&p, size_t n) : ptr((void **) &p), size(n) {}
+		void **ptr;
+		size_t size;
+	};
+	static size_t up(size_t x) { return (x + 255) & ~(size_t) 255; }
+	std::vector<Part> parts;
+	size_t			  bytes = 0;
+	StageLayout(std::initializer_list<Part> l) : parts(l) { for (const Part &p : parts) bytes += up(p.size); }
+	void place(void *base) const
+	{
+		char *b = (char *) base;
+		for (const Part &p : parts)
+		{
+			*p.ptr = b;
+			b += up(p.size);
+		}
+	}
+};
 
 static pgemb_status compute_norms(pgemb_index *idx, size_t first, size_t n, cudaStream_t s)
 {
@@ -499,8 +544,6 @@ static int env_int(const char *name, int dflt)
 	const char *v = getenv(name);
 	return (v && *v) ? atoi(v) : dflt;
 }
-
-static uint32_t align_up(uint32_t x, uint32_t a) { return (x + a - 1) / a * a; }
 
 // shared-memory layout + slots/rings per CTA: search_config.h (shared with the host emulation harness in tests/emu)
 static pgemb_status make_config(const pgemb_index *idx, uint32_t ef, SearchConfig *c, bool coop = false, bool res_global = false)
@@ -843,20 +886,24 @@ extern "C" pgemb_status pgemb_search_batch(pgemb_index *idx, size_t nq, const co
 	pgemb_status st = set_device(idx);
 	if (st) return st;
 	const size_t dim = idx->meta.dim;
-	const size_t qb = align_up((uint32_t) 0, 1) + nq * dim * sizeof(float);
 	const size_t lb = nq * ef * sizeof(uint64_t), db = nq * ef * sizeof(float), ib = nq * ef * sizeof(uint32_t);
 	const size_t nb = nq * sizeof(int32_t), sb = nq * 4 * sizeof(uint32_t);
-	auto		 up = [](size_t x) { return (x + 255) & ~(size_t) 255; };
-	const size_t total = up(qb) + up(lb) + up(db) + up(ib) + up(nb) + up(sb);
-	st = ensure_stage(idx, total);
+	float		*d_q = nullptr, *d_d = nullptr;
+	uint64_t	*d_l = nullptr;
+	uint32_t	*d_i = nullptr, *d_s = nullptr;
+	int32_t		*d_n = nullptr;
+	const StageLayout stage{{d_q, nq * dim * sizeof(float)}, {d_l, lb}, {d_d, db}, {d_i, ib}, {d_n, nb}, {d_s, sb}};
+	st = ensure_stage(idx, stage.bytes);
 	if (st) return st;
-	char	 *base = (char *) idx->d_stage;
-	float	 *d_q = (float *) base;				base += up(qb);
-	uint64_t *d_l = (uint64_t *) base;			base += up(lb);
-	float	 *d_d = (float *) base;				base += up(db);
-	uint32_t *d_i = (uint32_t *) base;			base += up(ib);
-	int32_t	 *d_n = (int32_t *) base;			base += up(nb);
-	uint32_t *d_s = (uint32_t *) base;
+	stage.place(idx->d_stage);
+	cudaStream_t s = idx->stream;
+	// the outputs the caller asked for, in staging order: [labels | dists | ids | counts | stats]
+	const struct { void *host; const void *dev; size_t bytes; } outs[5] = {{labels_out, d_l, lb}, {dists_out, d_d, db}, {ids_out, d_i, ib}, {n_out, d_n, nb}, {stats_out, d_s, sb}};
+	auto copy_out = [&]() -> pgemb_status {
+		for (const auto &o : outs)
+			if (o.host) CU_TRY(cudaMemcpyAsync(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost, s));
+		return PGEMB_OK;
+	};
 	// ONE traversal launch; the query batch is streamed in next to it: the copy stream moves chunk after chunk
 	// H2D and publishes "queries available" after each, the kernel's slots wait for their query to land
 	// (SearchParams::avail).  So the PCIe transfer hides behind the traversal instead of preceding it.
@@ -864,7 +911,6 @@ extern "C" pgemb_status pgemb_search_batch(pgemb_index *idx, size_t nq, const co
 	// blocking launch (CUDA_LAUNCH_BLOCKING, a profiler or sanitizer serialising kernels) cannot leave the kernel
 	// waiting for data that was never queued.  Under such a tool (detected by its injection variable) the batch is
 	// simply copied before the launch: replayed kernels must not depend on a concurrent copy.
-	cudaStream_t s = idx->stream;
 	if (env_int("PGEMB_FAST_SMALL", 1) != 0 && nq <= 64)
 	{
 		// a handful of queries (the reference-shaped hnsw_search: one) are not worth the streaming protocol
@@ -880,7 +926,7 @@ extern "C" pgemb_status pgemb_search_batch(pgemb_index *idx, size_t nq, const co
 		// the outputs are one contiguous range of the staging buffer [labels | dists | ids | counts | stats]: ONE copy into pinned
 		// memory + the 4-byte error flag, then one synchronisation (a copy into the caller's pageable buffers would block the host
 		// once per copy)
-		const size_t range = (size_t) ((char *) d_s - (char *) d_l) + up(sb);
+		const size_t range = (size_t) ((char *) d_s - (char *) d_l) + StageLayout::up(sb);
 		if (range + 64 <= ((size_t) 4 << 20))
 		{
 			if (idx->land_bytes < range + 64)
@@ -895,20 +941,13 @@ extern "C" pgemb_status pgemb_search_batch(pgemb_index *idx, size_t nq, const co
 			CU_TRY(cudaMemcpyAsync(idx->h_land, d_l, range, cudaMemcpyDeviceToHost, s));
 			CU_TRY(cudaMemcpyAsync(h_err, idx->d_error, sizeof(int), cudaMemcpyDeviceToHost, s));
 			CU_TRY(cudaStreamSynchronize(s));
-			const char *hb = idx->h_land;
-			if (labels_out) memcpy(labels_out, hb + ((char *) d_l - (char *) d_l), lb);
-			if (dists_out) memcpy(dists_out, hb + ((char *) d_d - (char *) d_l), db);
-			if (ids_out) memcpy(ids_out, hb + ((char *) d_i - (char *) d_l), ib);
-			memcpy(n_out, hb + ((char *) d_n - (char *) d_l), nb);
-			if (stats_out) memcpy(stats_out, hb + ((char *) d_s - (char *) d_l), sb);
+			for (const auto &o : outs)
+				if (o.host) memcpy(o.host, idx->h_land + ((const char *) o.dev - (const char *) d_l), o.bytes);
 			if (*h_err != 0) return check_device_error(idx, s);	 // reads, reports and clears the flag
 			return PGEMB_OK;
 		}
-		if (labels_out) CU_TRY(cudaMemcpyAsync(labels_out, d_l, lb, cudaMemcpyDeviceToHost, s));
-		if (dists_out) CU_TRY(cudaMemcpyAsync(dists_out, d_d, db, cudaMemcpyDeviceToHost, s));
-		if (ids_out) CU_TRY(cudaMemcpyAsync(ids_out, d_i, ib, cudaMemcpyDeviceToHost, s));
-		CU_TRY(cudaMemcpyAsync(n_out, d_n, nb, cudaMemcpyDeviceToHost, s));
-		if (stats_out) CU_TRY(cudaMemcpyAsync(stats_out, d_s, sb, cudaMemcpyDeviceToHost, s));
+		st = copy_out();
+		if (st) return st;
 		return check_device_error(idx, s);
 	}
 	if (!idx->s_in)
@@ -957,11 +996,8 @@ extern "C" pgemb_status pgemb_search_batch(pgemb_index *idx, size_t nq, const co
 		cudaStreamSynchronize(idx->s_in);
 		return st;
 	}
-	if (labels_out) CU_TRY(cudaMemcpyAsync(labels_out, d_l, lb, cudaMemcpyDeviceToHost, s));
-	if (dists_out) CU_TRY(cudaMemcpyAsync(dists_out, d_d, db, cudaMemcpyDeviceToHost, s));
-	if (ids_out) CU_TRY(cudaMemcpyAsync(ids_out, d_i, ib, cudaMemcpyDeviceToHost, s));
-	CU_TRY(cudaMemcpyAsync(n_out, d_n, nb, cudaMemcpyDeviceToHost, s));
-	if (stats_out) CU_TRY(cudaMemcpyAsync(stats_out, d_s, sb, cudaMemcpyDeviceToHost, s));
+	st = copy_out();
+	if (st) return st;
 	CU_TRY(cudaStreamSynchronize(idx->s_in));
 	return check_device_error(idx, s);
 }
@@ -995,16 +1031,12 @@ static pgemb_status launch_pairs(int metric, const float *d_a, const float *d_b,
 	const uint32_t threads = 128;
 	const uint32_t lanes = (metric == DIST_L2) ? 8 : 4;
 	const uint32_t blocks = (uint32_t) (((size_t) n * lanes + threads - 1) / threads);
-	switch (metric)
-	{
-		case DIST_L2: PGEMB_LAUNCH(dist_pairs_kernel<M_L2>, blocks, threads, 0, s, d_a, d_b, dim, dim, dim, n, broadcast_a, d_out); break;
-		case DIST_COSINE: PGEMB_LAUNCH(dist_pairs_kernel<M_COS>, blocks, threads, 0, s, d_a, d_b, dim, dim, dim, n, broadcast_a, d_out); break;
-		case DIST_MANHATTAN: PGEMB_LAUNCH(dist_pairs_kernel<M_MAN>, blocks, threads, 0, s, d_a, d_b, dim, dim, dim, n, broadcast_a, d_out); break;
-		default: return fail(PGEMB_ERR_ARG, "unknown distance function");
-	}
-	g_launches++;
-	CU_TRY(cudaGetLastError());
-	return PGEMB_OK;
+	return with_metric(metric, [&](auto m) -> pgemb_status {
+		PGEMB_LAUNCH(dist_pairs_kernel<decltype(m)::value>, blocks, threads, 0, s, d_a, d_b, dim, dim, dim, n, broadcast_a, d_out);
+		g_launches++;
+		CU_TRY(cudaGetLastError());
+		return PGEMB_OK;
+	});
 }
 
 // hnsw_dist_func has no handle to hang a buffer on (distfunc.c:171: two pointers and a length), so the staging area of the
@@ -1028,11 +1060,11 @@ extern "C" pgemb_status pgemb_dist_batch(dist_func_t dist, size_t dim, size_t n,
 	if (n >= (1ull << 28)) return fail(PGEMB_ERR_ARG, "batch too large");
 	int dev = 0;
 	CU_TRY(cudaGetDevice(&dev));
-	auto		 up = [](size_t x) { return (x + 255) & ~(size_t) 255; };
 	const size_t ab = (broadcast_a ? 1 : n) * dim * sizeof(float), bb = n * dim * sizeof(float), ob = n * sizeof(float);
-	const size_t total = up(ab) + up(bb) + up(ob);
+	float		*d_a = nullptr, *d_b = nullptr, *d_o = nullptr;
+	const StageLayout stage{{d_a, ab}, {d_b, bb}, {d_o, ob}};
 	std::lock_guard<std::mutex> lock(g_pair_stage.mu);
-	if (g_pair_stage.device != dev || g_pair_stage.bytes < total)
+	if (g_pair_stage.device != dev || g_pair_stage.bytes < stage.bytes)
 	{
 		if (g_pair_stage.d)
 		{
@@ -1047,7 +1079,7 @@ extern "C" pgemb_status pgemb_dist_batch(dist_func_t dist, size_t dim, size_t n,
 		}
 		g_pair_stage.d = nullptr;
 		g_pair_stage.bytes = 0;
-		const size_t want = total + total / 2 + 65536;
+		const size_t want = stage.bytes + stage.bytes / 2 + 65536;
 		if (cudaMalloc(&g_pair_stage.d, want) != cudaSuccess)
 		{
 			cudaGetLastError();
@@ -1057,8 +1089,7 @@ extern "C" pgemb_status pgemb_dist_batch(dist_func_t dist, size_t dim, size_t n,
 		g_pair_stage.bytes = want;
 		g_pair_stage.device = dev;
 	}
-	char  *base = (char *) g_pair_stage.d;
-	float *d_a = (float *) base, *d_b = (float *) (base + up(ab)), *d_o = (float *) (base + up(ab) + up(bb));
+	stage.place(g_pair_stage.d);
 	CU_TRY(cudaMemcpyAsync(d_a, a, ab, cudaMemcpyHostToDevice, 0));
 	CU_TRY(cudaMemcpyAsync(d_b, b, bb, cudaMemcpyHostToDevice, 0));
 	pgemb_status st = launch_pairs((int) dist, d_a, d_b, (uint32_t) dim, (uint32_t) n, broadcast_a, d_o, 0);
@@ -1075,27 +1106,25 @@ extern "C" pgemb_status pgemb_dist_gather(pgemb_index *idx, size_t nq, const coo
 	pgemb_status st = set_device(idx);
 	if (st) return st;
 	const size_t dim = idx->meta.dim;
-	auto		 up = [](size_t x) { return (x + 255) & ~(size_t) 255; };
 	const size_t qb = nq * dim * 4, ib = nq * k * 4, ob = nq * k * 4;
-	st = ensure_stage(idx, up(qb) + up(ib) + up(ob));
+	float		*d_q = nullptr, *d_o = nullptr;
+	uint32_t	*d_i = nullptr;
+	const StageLayout stage{{d_q, qb}, {d_i, ib}, {d_o, ob}};
+	st = ensure_stage(idx, stage.bytes);
 	if (st) return st;
-	char		*base = (char *) idx->d_stage;
-	float		*d_q = (float *) base;		base += up(qb);
-	uint32_t	*d_i = (uint32_t *) base;	base += up(ib);
-	float		*d_o = (float *) base;
+	stage.place(idx->d_stage);
 	cudaStream_t s = idx->stream;
 	CU_TRY(cudaMemcpyAsync(d_q, queries, qb, cudaMemcpyHostToDevice, s));
 	CU_TRY(cudaMemcpyAsync(d_i, ids, ib, cudaMemcpyHostToDevice, s));
 	const int	   metric = (int) idx->meta.dist_func;
 	const uint32_t threads = 128, lanes = (metric == DIST_L2) ? 8 : 4;
 	const uint32_t blocks = (uint32_t) ((nq * k * lanes + threads - 1) / threads);
-#define GATHER(MM)                                                                                                              \
-	PGEMB_LAUNCH(dist_gather_kernel<MM>, blocks, threads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim, (uint32_t) idx->n, d_q, \
-													  (uint32_t) dim, (uint32_t) nq, (uint32_t) k, d_i, d_o)
-	if (metric == DIST_L2) GATHER(M_L2);
-	else if (metric == DIST_COSINE) GATHER(M_COS);
-	else GATHER(M_MAN);
-#undef GATHER
+	st = with_metric(metric, [&](auto m) -> pgemb_status {
+		PGEMB_LAUNCH(dist_gather_kernel<decltype(m)::value>, blocks, threads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim,
+					 (uint32_t) idx->n, d_q, (uint32_t) dim, (uint32_t) nq, (uint32_t) k, d_i, d_o);
+		return PGEMB_OK;
+	});
+	if (st) return st;
 	g_launches++;
 	CU_TRY(cudaGetLastError());
 	CU_TRY(cudaMemcpyAsync(out, d_o, ob, cudaMemcpyDeviceToHost, s));
@@ -1199,9 +1228,11 @@ static pgemb_status launch_scan_filter(pgemb_index *idx, int metric, const float
 #ifdef PGEMB_HOST_EMULATION
 	(void) s;
 	(void) d_qn;
-	if (metric == DIST_L2) scan_filter_emulated<M_L2>(d_q, idx->row_f, idx->d_vectors, idx->row_f, (uint32_t) idx->meta.dim, rel, d_qn, p);
-	else scan_filter_emulated<M_COS>(d_q, idx->row_f, idx->d_vectors, idx->row_f, (uint32_t) idx->meta.dim, rel, d_qn, p);
-	g_launches++;
+	return with_tc_metric(metric, [&](auto m) -> pgemb_status {
+		scan_filter_emulated<decltype(m)::value>(d_q, idx->row_f, idx->d_vectors, idx->row_f, (uint32_t) idx->meta.dim, rel, d_qn, p);
+		g_launches++;
+		return PGEMB_OK;
+	});
 #else
 	(void) rel;
 	(void) d_qn;
@@ -1212,20 +1243,14 @@ static pgemb_status launch_scan_filter(pgemb_index *idx, int metric, const float
 	if (st) return st;
 	const uint32_t tiles = p.n_qtiles * p.n_rtiles;
 	const uint32_t grid = tiles < (uint32_t) idx->sm_count ? tiles : (uint32_t) idx->sm_count;
-	if (metric == DIST_L2)
-	{
-		CU_TRY(cudaFuncSetAttribute(scan_filter_wgmma_kernel<M_L2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kUmmaSmem));
-		scan_filter_wgmma_kernel<M_L2><<<grid, kUmmaThreads, kUmmaSmem, s>>>(tq, tv, p);
-	}
-	else
-	{
-		CU_TRY(cudaFuncSetAttribute(scan_filter_wgmma_kernel<M_COS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kUmmaSmem));
-		scan_filter_wgmma_kernel<M_COS><<<grid, kUmmaThreads, kUmmaSmem, s>>>(tq, tv, p);
-	}
-	g_launches++;
-	CU_TRY(cudaGetLastError());
+	return with_tc_metric(metric, [&](auto m) -> pgemb_status {
+		CU_TRY(cudaFuncSetAttribute(scan_filter_wgmma_kernel<decltype(m)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kUmmaSmem));
+		scan_filter_wgmma_kernel<decltype(m)::value><<<grid, kUmmaThreads, kUmmaSmem, s>>>(tq, tv, p);
+		g_launches++;
+		CU_TRY(cudaGetLastError());
+		return PGEMB_OK;
+	});
 #endif
-	return PGEMB_OK;
 }
 
 static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
@@ -1306,7 +1331,6 @@ static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *q
 	const size_t dim = idx->meta.dim;
 	const size_t N = idx->n;
 	const size_t rf = idx->row_f;
-	auto		 up = [](size_t x) { return (x + 255) & ~(size_t) 255; };
 	const bool	 tc = scan_use_tc(idx, allow_tc);
 	const int	 metric = (int) idx->meta.dist_func;
 	cudaStream_t s = idx->stream;
@@ -1330,22 +1354,17 @@ static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *q
 	}
 	const size_t qb = nq * rf * 4, db = tc ? 0 : nq * chunk * 4, kd = nq * k * 4, kl = nq * k * 8, nb = nq * 4;
 	const size_t cb = tc ? nq * cap * 4 : 0;
-	st = ensure_stage(idx, up(qb) + up(db) + 2 * up(kd) + 2 * up(kl) + 3 * up(nb) + up(nq * 8) + 2 * up(cb) + 512);
+	float	 *d_q = nullptr, *d_dist = nullptr, *d_qn = nullptr, *d_cs = nullptr;
+	uint32_t *d_td = nullptr, *d_sd = nullptr, *d_tn = nullptr, *d_cn = nullptr, *d_cr = nullptr, *d_cnt = nullptr;
+	uint64_t *d_tl = nullptr, *d_sl = nullptr;
+	float2	 *d_qc = nullptr;
+	// d_q: [nq][row_f], zero padded (the TMA tensor map reads whole 16-byte units); d_cn, d_qc, d_cr, d_cs: candidate counts, filter
+	// constants, candidate rows, candidate products; d_cnt: [0] re-scored, [1] tripwire, [2] overflowed queries
+	const StageLayout stage{{d_q, qb}, {d_dist, db}, {d_td, kd}, {d_sd, kd}, {d_tl, kl}, {d_sl, kl}, {d_tn, nb},
+							{d_qn, nb}, {d_cn, nb}, {d_qc, nq * 8}, {d_cr, cb}, {d_cs, cb}, {d_cnt, 16}};
+	st = ensure_stage(idx, stage.bytes + 256);
 	if (st) return st;
-	char	 *base = (char *) idx->d_stage;
-	float	 *d_q = (float *) base;			base += up(qb);		// [nq][row_f], zero padded (the TMA tensor map reads whole 16-byte units)
-	float	 *d_dist = (float *) base;		base += up(db);
-	uint32_t *d_td = (uint32_t *) base;		base += up(kd);
-	uint32_t *d_sd = (uint32_t *) base;		base += up(kd);
-	uint64_t *d_tl = (uint64_t *) base;		base += up(kl);
-	uint64_t *d_sl = (uint64_t *) base;		base += up(kl);
-	uint32_t *d_tn = (uint32_t *) base;		base += up(nb);
-	float	 *d_qn = (float *) base;		base += up(nb);
-	uint32_t *d_cn = (uint32_t *) base;		base += up(nb);		// candidate counts
-	float2	 *d_qc = (float2 *) base;		base += up(nq * 8);	// filter constants
-	uint32_t *d_cr = (uint32_t *) base;		base += up(cb);		// candidate rows
-	float	 *d_cs = (float *) base;		base += up(cb);		// candidate products
-	uint32_t *d_cnt = (uint32_t *) base;						// [0] re-scored, [1] tripwire, [2] overflowed queries
+	stage.place(idx->d_stage);
 	if (rf != dim) CU_TRY(cudaMemsetAsync(d_q, 0, qb, s));
 	CU_TRY(cudaMemcpy2DAsync(d_q, rf * 4, queries, dim * 4, dim * 4, nq, device_io ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
 	CU_TRY(cudaMemsetAsync(d_tn, 0, nb, s));
@@ -1385,8 +1404,11 @@ static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *q
 		if (st) return st;
 		const float rel = scan_tc_rel(dim);
 		CU_TRY(cudaMemsetAsync(d_cnt, 0, 16, s));
-		if (metric == DIST_L2) PGEMB_LAUNCH(scan_qconst_init_kernel<M_L2>, (uint32_t) ((nq + 127) / 128), 128, 0, s, d_qn, (uint32_t) nq, rel, d_qc, d_cn);
-		else PGEMB_LAUNCH(scan_qconst_init_kernel<M_COS>, (uint32_t) ((nq + 127) / 128), 128, 0, s, d_qn, (uint32_t) nq, rel, d_qc, d_cn);
+		st = with_tc_metric(metric, [&](auto m) -> pgemb_status {
+			PGEMB_LAUNCH(scan_qconst_init_kernel<decltype(m)::value>, (uint32_t) ((nq + 127) / 128), 128, 0, s, d_qn, (uint32_t) nq, rel, d_qc, d_cn);
+			return PGEMB_OK;
+		});
+		if (st) return st;
 		g_launches++;
 		size_t csize = c0;
 		size_t growth = (size_t) env_int("PGEMB_SCAN_TC_GROWTH", 2);	// measured (profiles/r2_call10_scan_growth_sweep.log): 2 / 3 / 4 / 8 -> 6.7 / 7.7 / 8.0 / 8.6 ms per 1024 x 1M x 768 scan at k 64
@@ -1404,12 +1426,13 @@ static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *q
 			if (N - r0 - nr < nr / 8) nr = N - r0;	// do not leave a sliver for an extra launch pair
 			st = launch_scan_filter(idx, metric, d_q, d_qn, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, rel, d_qc, d_cr, d_cs, d_cn, (uint32_t) cap, nullptr, s);
 			if (st) return st;
-#define SCAN_RESCORE(MM)                                                                                                                          \
-	PGEMB_LAUNCH(scan_rescore_kernel<MM>, (uint32_t) nq, 128, 0, s, idx->d_vectors, idx->row_f, (uint32_t) dim, idx->d_norms, d_q, (uint32_t) rf, d_qn,  \
-				 idx->d_labels, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, (uint32_t) k, rel, d_cr, d_cs, d_cn, (uint32_t) cap, d_td, d_tl, d_tn, d_sd, d_sl, d_qc, d_cnt)
-			if (metric == DIST_L2) { SCAN_RESCORE(M_L2); }
-			else { SCAN_RESCORE(M_COS); }
-#undef SCAN_RESCORE
+			st = with_tc_metric(metric, [&](auto m) -> pgemb_status {
+				PGEMB_LAUNCH(scan_rescore_kernel<decltype(m)::value>, (uint32_t) nq, 128, 0, s, idx->d_vectors, idx->row_f, (uint32_t) dim, idx->d_norms, d_q,
+							 (uint32_t) rf, d_qn, idx->d_labels, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, (uint32_t) k, rel, d_cr, d_cs, d_cn, (uint32_t) cap,
+							 d_td, d_tl, d_tn, d_sd, d_sl, d_qc, d_cnt);
+				return PGEMB_OK;
+			});
+			if (st) return st;
 			g_launches++;
 			CU_TRY(cudaGetLastError());
 			r0 += nr;
@@ -1428,23 +1451,18 @@ static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *q
 			const size_t   nr = (N - r0 < chunk) ? (N - r0) : chunk;
 			const uint32_t threads = 128;
 			const uint32_t blocks = (uint32_t) ((nq * nr * lanes + threads - 1) / threads);
-#define SCAN_DIST(MM)                                                                                                              \
-	PGEMB_LAUNCH(scan_dist_kernel<MM>, blocks, threads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim, d_q, (uint32_t) rf, \
-													(uint32_t) nq, (uint32_t) r0, (uint32_t) nr, d_dist)
-#define SCAN_TILE(MM)                                                                                                              \
-	PGEMB_LAUNCH(scan_tile_kernel<MM>, dim3((uint32_t) ((nq + ScanTile<MM>::TQ - 1) / ScanTile<MM>::TQ), (uint32_t) ((nr + kScanTileRows - 1) / kScanTileRows)), kScanThreads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim, d_q, (uint32_t) rf, d_qn,  \
-												 (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, d_dist)
-			if (tiled)
-			{
-				if (metric == DIST_L2) SCAN_TILE(M_L2);
-				else if (metric == DIST_COSINE) SCAN_TILE(M_COS);
-				else SCAN_TILE(M_MAN);
-			}
-			else if (metric == DIST_L2) SCAN_DIST(M_L2);
-			else if (metric == DIST_COSINE) SCAN_DIST(M_COS);
-			else SCAN_DIST(M_MAN);
-#undef SCAN_TILE
-#undef SCAN_DIST
+			st = with_metric(metric, [&](auto m) -> pgemb_status {
+				constexpr uint32_t tq = ScanTile<decltype(m)::value>::TQ;
+				if (tiled)
+					PGEMB_LAUNCH(scan_tile_kernel<decltype(m)::value>, dim3((uint32_t) ((nq + tq - 1) / tq), (uint32_t) ((nr + kScanTileRows - 1) / kScanTileRows)),
+								 kScanThreads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim, d_q, (uint32_t) rf, d_qn, (uint32_t) nq,
+								 (uint32_t) r0, (uint32_t) nr, d_dist);
+				else
+					PGEMB_LAUNCH(scan_dist_kernel<decltype(m)::value>, blocks, threads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim, d_q,
+								 (uint32_t) rf, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, d_dist);
+				return PGEMB_OK;
+			});
+			if (st) return st;
 			PGEMB_LAUNCH(scan_select_kernel, (uint32_t) ((nq + 3) / 4), 128, 0, s, d_dist, idx->d_labels, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, (uint32_t) k,
 																		 d_td, d_tl, d_tn, d_sd, d_sl);
 			g_launches += 2;
@@ -1521,15 +1539,13 @@ extern "C" pgemb_status pgemb_debug_umma_product(pgemb_index *idx, size_t nq, co
 	if (nq * nr > ((size_t) 1 << 28)) return fail(PGEMB_ERR_ARG, "debug product too large");
 	pgemb_status st = set_device(idx);
 	if (st) return st;
-	auto		 up = [](size_t x) { return (x + 255) & ~(size_t) 255; };
 	const size_t rf = idx->row_f, dim = idx->meta.dim;
-	st = ensure_stage(idx, up(nq * rf * 4) + up(nq * 4) + up(nq * nr * 4) + 256);
+	float		*d_q = nullptr, *d_qn = nullptr, *d_s = nullptr;
+	const StageLayout stage{{d_q, nq * rf * 4}, {d_qn, nq * 4}, {d_s, nq * nr * 4}};
+	st = ensure_stage(idx, stage.bytes + 256);
 	if (st) return st;
+	stage.place(idx->d_stage);
 	cudaStream_t s = idx->stream;
-	char		*base = (char *) idx->d_stage;
-	float		*d_q = (float *) base;	base += up(nq * rf * 4);
-	float		*d_qn = (float *) base;	base += up(nq * 4);
-	float		*d_s = (float *) base;
 	CU_TRY(cudaMemsetAsync(d_q, 0, nq * rf * 4, s));
 	CU_TRY(cudaMemcpy2DAsync(d_q, rf * 4, queries, dim * 4, dim * 4, nq, cudaMemcpyHostToDevice, s));
 	CU_TRY(cudaMemsetAsync(d_s, 0, nq * nr * 4, s));
@@ -1808,40 +1824,32 @@ static GraphView graph_view(pgemb_index *idx)
 	return g;
 }
 
-// Connect `count` new nodes whose candidate lists sit in bind_ws slots [0,count): select + back-links.
-static pgemb_status launch_connect(pgemb_index *idx, const uint32_t *d_new_ids, size_t count, size_t ef, cudaStream_t s)
+// Select: each of `count` new nodes whose candidate lists sit in bind_ws slots [0,count) picks its neighbours and writes its
+// (target, source) pairs to bind_ws.d_pairs.  `staged`: the heuristic with its operands staged in shared memory.
+static pgemb_status launch_select(pgemb_index *idx, const uint32_t *d_new_ids, size_t count, size_t ef, bool staged, cudaStream_t s)
 {
-	BindWorkspace &w = idx->bind_ws;
-	GraphView	   g = graph_view(idx);
-	const size_t   M = idx->meta.M ? idx->meta.M : 1;
-	const size_t   maxM1 = idx->meta.maxM + 1;
-	// a handful of inserts (hnsw_bind_point: one): the heuristic with its operands staged in shared memory -- the kept rows
-	// must fit next to the key arrays (M = 32 at 768-d: 100 KB); batches keep the small-footprint kernel (many CTAs per SM)
-	const size_t   sel_staged_bytes = select_smem_bytes(ef, M, idx->row_f, true);
-	const bool	   staged = count <= 8 && M <= 256 && sel_staged_bytes <= 200 * 1024 && env_int("PGEMB_SELECT_STAGED", 1) != 0;
-	const size_t   sel_smem = staged ? sel_staged_bytes : select_smem_bytes(ef, M, idx->row_f, false);
-	const size_t   bl_smem = maxM1 * 8 * 2 + (idx->meta.maxM ? idx->meta.maxM : 1) * 8 + maxM1 * 4;
-	const int	   metric = (int) idx->meta.dist_func;
-#define LAUNCH_SELECT(MM)                                                                                                        \
-	do {                                                                                                                         \
-		if (staged)                                                                                                              \
-		{                                                                                                                        \
-			if (sel_smem > 48 * 1024) CU_TRY(cudaFuncSetAttribute(select_kernel<MM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sel_smem)); \
-			PGEMB_LAUNCH((select_kernel<MM, true>), (uint32_t) count, kBindThreads, sel_smem, s, g, d_new_ids, w.d_cand_ids, w.d_cand_d, w.d_cand_n, (uint32_t) ef, w.d_pairs); \
-		}                                                                                                                        \
-		else                                                                                                                     \
-		{                                                                                                                        \
-			if (sel_smem > 48 * 1024) CU_TRY(cudaFuncSetAttribute(select_kernel<MM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sel_smem)); \
-			PGEMB_LAUNCH(select_kernel<MM>, (uint32_t) count, kBindThreads, sel_smem, s, g, d_new_ids, w.d_cand_ids, w.d_cand_d, w.d_cand_n, (uint32_t) ef, w.d_pairs); \
-		}                                                                                                                        \
-	} while (0)
-	if (metric == DIST_L2) LAUNCH_SELECT(M_L2);
-	else if (metric == DIST_COSINE) LAUNCH_SELECT(M_COS);
-	else LAUNCH_SELECT(M_MAN);
-#undef LAUNCH_SELECT
-	g_launches++;
-	CU_TRY(cudaGetLastError());
-	const size_t   n_pairs = count * M;
+	BindWorkspace  &w = idx->bind_ws;
+	const GraphView g = graph_view(idx);
+	const size_t	sel_smem = select_smem_bytes(ef, idx->meta.M, idx->row_f, staged);
+	return with_metric((int) idx->meta.dist_func, [&](auto m) -> pgemb_status {
+		const auto fn = staged ? select_kernel<decltype(m)::value, true> : select_kernel<decltype(m)::value, false>;
+		if (sel_smem > 48 * 1024) CU_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sel_smem));
+		PGEMB_LAUNCH(fn, (uint32_t) count, kBindThreads, sel_smem, s, g, d_new_ids, w.d_cand_ids, w.d_cand_d, w.d_cand_n, (uint32_t) ef, w.d_pairs);
+		g_launches++;
+		CU_TRY(cudaGetLastError());
+		return PGEMB_OK;
+	});
+}
+
+// Back-links of the pairs of the first `count` selected nodes: sorted by (target, source), so that every target takes its new
+// neighbours in source-id order -- the sequential order.
+static pgemb_status launch_backlinks(pgemb_index *idx, size_t count, cudaStream_t s)
+{
+	BindWorkspace  &w = idx->bind_ws;
+	const GraphView g = graph_view(idx);
+	const size_t	maxM1 = idx->meta.maxM + 1;
+	const size_t	bl_smem = maxM1 * 8 * 2 + (idx->meta.maxM ? idx->meta.maxM : 1) * 8 + maxM1 * 4;
+	const uint32_t	n_pairs = (uint32_t) (count * (idx->meta.M ? idx->meta.M : 1));
 	const uint64_t *sorted = w.d_pairs;
 	if (count > 1)
 	{
@@ -1850,18 +1858,25 @@ static pgemb_status launch_connect(pgemb_index *idx, const uint32_t *d_new_ids, 
 		g_launches++;
 		sorted = w.d_pairs_sorted;
 	}
-#define LAUNCH_BACK(MM)                                                                                                          \
-	do {                                                                                                                         \
-		if (bl_smem > 48 * 1024) CU_TRY(cudaFuncSetAttribute(backlink_kernel<MM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) bl_smem)); \
-		PGEMB_LAUNCH(backlink_kernel<MM>, (uint32_t) n_pairs, kBindThreads, bl_smem, s, g, sorted, (uint32_t) n_pairs);                      \
-	} while (0)
-	if (metric == DIST_L2) LAUNCH_BACK(M_L2);
-	else if (metric == DIST_COSINE) LAUNCH_BACK(M_COS);
-	else LAUNCH_BACK(M_MAN);
-#undef LAUNCH_BACK
-	g_launches++;
-	CU_TRY(cudaGetLastError());
-	return PGEMB_OK;
+	return with_metric((int) idx->meta.dist_func, [&](auto m) -> pgemb_status {
+		if (bl_smem > 48 * 1024) CU_TRY(cudaFuncSetAttribute(backlink_kernel<decltype(m)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) bl_smem));
+		PGEMB_LAUNCH(backlink_kernel<decltype(m)::value>, n_pairs, kBindThreads, bl_smem, s, g, sorted, n_pairs);
+		g_launches++;
+		CU_TRY(cudaGetLastError());
+		return PGEMB_OK;
+	});
+}
+
+// Connect `count` new nodes whose candidate lists sit in bind_ws slots [0,count): select + back-links.
+static pgemb_status launch_connect(pgemb_index *idx, const uint32_t *d_new_ids, size_t count, size_t ef, cudaStream_t s)
+{
+	// a handful of inserts (hnsw_bind_point: one): the heuristic with its operands staged in shared memory -- the kept rows
+	// must fit next to the key arrays (M = 32 at 768-d: 100 KB); batches keep the small-footprint kernel (many CTAs per SM)
+	const size_t M = idx->meta.M ? idx->meta.M : 1;
+	const bool	 staged = count <= 8 && M <= 256 && select_smem_bytes(ef, M, idx->row_f, true) <= 200 * 1024 && env_int("PGEMB_SELECT_STAGED", 1) != 0;
+	pgemb_status st = launch_select(idx, d_new_ids, count, ef, staged, s);
+	if (st) return st;
+	return launch_backlinks(idx, count, s);
 }
 
 __global__ void iota_kernel(uint32_t *out, uint32_t start, uint32_t n);
@@ -1901,16 +1916,27 @@ pgemb_status bind_points(pgemb_index *idx, idx_t first, size_t n)
 	return PGEMB_OK;
 }
 
-// two timing events that go away on every return path
-struct EventPair
+// device time of a build from start() to finish(); the two events go away on every return path
+struct BuildTimer
 {
 	cudaEvent_t e0 = nullptr, e1 = nullptr;
-	cudaError_t create()
+	cudaError_t start(cudaStream_t s)
 	{
 		cudaError_t e = cudaEventCreate(&e0);
-		return e != cudaSuccess ? e : cudaEventCreate(&e1);
+		if (e == cudaSuccess) e = cudaEventCreate(&e1);
+		return e != cudaSuccess ? e : cudaEventRecord(e0, s);
 	}
-	~EventPair()
+	// the build is enqueued: waits for it, returns the kernels' sticky error and its device seconds in *seconds_out
+	pgemb_status finish(pgemb_index *idx, cudaStream_t s, double *seconds_out)
+	{
+		CU_TRY(cudaEventRecord(e1, s));
+		const pgemb_status st = check_device_error(idx, s);
+		float ms = 0.f;
+		cudaEventElapsedTime(&ms, e0, e1);
+		if (seconds_out) *seconds_out = ms * 1e-3;
+		return st;
+	}
+	~BuildTimer()
 	{
 		if (e0) cudaEventDestroy(e0);
 		if (e1) cudaEventDestroy(e1);
@@ -1937,10 +1963,8 @@ extern "C" pgemb_status pgemb_build_bulk(pgemb_index *idx, size_t first, size_t 
 	st = ensure_bind_ws(idx, batch_max, efc);
 	if (st) return st;
 	BindWorkspace &w = idx->bind_ws;
-	EventPair ev;
-	CU_TRY(ev.create());
-	const cudaEvent_t e0 = ev.e0, e1 = ev.e1;
-	CU_TRY(cudaEventRecord(e0, s));
+	BuildTimer	   timer;
+	CU_TRY(timer.start(s));
 	size_t pos = first;
 	const size_t end = first + n;
 	while (pos < end)
@@ -1963,12 +1987,7 @@ extern "C" pgemb_status pgemb_build_bulk(pgemb_index *idx, size_t first, size_t 
 		if (st) return st;
 		pos += B;
 	}
-	CU_TRY(cudaEventRecord(e1, s));
-	st = check_device_error(idx, s);
-	float ms = 0.f;
-	cudaEventElapsedTime(&ms, e0, e1);
-	if (seconds_out) *seconds_out = ms * 1e-3;
-	return st;
+	return timer.finish(idx, s, seconds_out);
 }
 
 // Exact AND parallel build: the result is bit-identical to n sequential hnsw_add_point calls (embedding.c:606-701).
@@ -2008,10 +2027,8 @@ extern "C" pgemb_status pgemb_build_exact(pgemb_index *idx, size_t first, size_t
 		w.stamp_cap = idx->capacity;
 	}
 	const size_t M = idx->meta.M ? idx->meta.M : 1;
-	EventPair ev;
-	CU_TRY(ev.create());
-	const cudaEvent_t e0 = ev.e0, e1 = ev.e1;
-	CU_TRY(cudaEventRecord(e0, s));
+	BuildTimer	 timer;
+	CU_TRY(timer.start(s));
 	size_t	 pos = first;
 	const size_t end = first + n;
 	size_t	 B = 1;
@@ -2033,20 +2050,9 @@ extern "C" pgemb_status pgemb_build_exact(pgemb_index *idx, size_t first, size_t
 		batches++;
 		searches += B;
 		size_t acc = B;
-		GraphView g = graph_view(idx);
-		const int metric = (int) idx->meta.dist_func;
-		const size_t sel_smem = efc * 8 + M * 8 + efc * 4;
-#define LAUNCH_SELECT_X(MM)                                                                                                     \
-	do {                                                                                                                         \
-		if (sel_smem > 48 * 1024) CU_TRY(cudaFuncSetAttribute(select_kernel<MM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sel_smem)); \
-		PGEMB_LAUNCH(select_kernel<MM>, (uint32_t) B, kBindThreads, sel_smem, s, g, w.d_qids, w.d_cand_ids, w.d_cand_d, w.d_cand_n, (uint32_t) efc, w.d_pairs); \
-	} while (0)
-		if (metric == DIST_L2) LAUNCH_SELECT_X(M_L2);
-		else if (metric == DIST_COSINE) LAUNCH_SELECT_X(M_COS);
-		else LAUNCH_SELECT_X(M_MAN);
-#undef LAUNCH_SELECT_X
-		g_launches++;
-		CU_TRY(cudaGetLastError());
+		// the small-footprint select at every batch size (launch_connect stages batches of up to 8)
+		st = launch_select(idx, w.d_qids, B, efc, false, s);
+		if (st) return st;
 		const uint32_t n_pairs_all = (uint32_t) (B * M);
 		if (B > 1)
 		{
@@ -2066,29 +2072,9 @@ extern "C" pgemb_status pgemb_build_exact(pgemb_index *idx, size_t first, size_t
 				g_launches++;
 			}
 		}
-		// back-links of the accepted prefix, per target in source order
-		const uint32_t	n_pairs = (uint32_t) (acc * M);
-		const uint64_t *sorted = w.d_pairs;
-		if (acc > 1)
-		{
-			size_t bytes = w.cub_bytes;
-			CU_TRY(cub::DeviceRadixSort::SortKeys(w.d_cub, bytes, w.d_pairs, w.d_pairs_sorted, (int) n_pairs, 0, 64, s));
-			g_launches++;
-			sorted = w.d_pairs_sorted;
-		}
-		const size_t maxM1 = idx->meta.maxM + 1;
-		const size_t bl_smem = maxM1 * 8 * 2 + (idx->meta.maxM ? idx->meta.maxM : 1) * 8 + maxM1 * 4;
-#define LAUNCH_BACK_X(MM)                                                                                                        \
-	do {                                                                                                                         \
-		if (bl_smem > 48 * 1024) CU_TRY(cudaFuncSetAttribute(backlink_kernel<MM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) bl_smem)); \
-		PGEMB_LAUNCH(backlink_kernel<MM>, n_pairs, kBindThreads, bl_smem, s, g, sorted, n_pairs);                                          \
-	} while (0)
-		if (metric == DIST_L2) LAUNCH_BACK_X(M_L2);
-		else if (metric == DIST_COSINE) LAUNCH_BACK_X(M_COS);
-		else LAUNCH_BACK_X(M_MAN);
-#undef LAUNCH_BACK_X
-		g_launches++;
-		CU_TRY(cudaGetLastError());
+		// back-links of the accepted prefix
+		st = launch_backlinks(idx, acc, s);
+		if (st) return st;
 		pos += acc;
 		// Speculative searches are nearly free (one launch, one warp each, latency-bound), so the batch only
 		// shrinks while the graph is tiny (every search expands most of it and everything conflicts).
@@ -2099,18 +2085,13 @@ extern "C" pgemb_status pgemb_build_exact(pgemb_index *idx, size_t first, size_t
 		// the sequential graph).
 		if (env_int("PGEMB_EXACT_CLAMP_SMS", 1) != 0 && B > (size_t) idx->sm_count && B <= 3 * (size_t) idx->sm_count) B = (size_t) idx->sm_count;
 	}
-	CU_TRY(cudaEventRecord(e1, s));
-	st = check_device_error(idx, s);
-	float ms = 0.f;
-	cudaEventElapsedTime(&ms, e0, e1);
-	if (seconds_out) *seconds_out = ms * 1e-3;
 	if (stats_out)
 	{
 		stats_out[0] = batches;
 		stats_out[1] = searches;
 		stats_out[2] = n;
 	}
-	return st;
+	return timer.finish(idx, s, seconds_out);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2148,6 +2129,28 @@ extern "C" pgemb_status pgemb_merge_topk_device(size_t nq, size_t n_shards, size
 }
 
 // One packed result buffer per rank: [labels u64 nq*k | dists f32 nq*k | counts i32 nq] -- what ONE all-gather moves.
+struct PackedTopk
+{
+	uint64_t *labels;
+	float	 *dists;
+	int32_t	 *counts;
+};
+
+static PackedTopk packed_topk(const void *base, size_t nq, size_t k)
+{
+	char *b = (char *) base;
+	return {(uint64_t *) b, (float *) (b + nq * k * 8), (int32_t *) (b + nq * k * 12)};
+}
+
+// a packed buffer as one input of the merge kernel
+static void set_shard(ShardLists &in, size_t shard, const void *base, size_t nq, size_t k)
+{
+	const PackedTopk p = packed_topk(base, nq, k);
+	in.lab[shard] = p.labels;
+	in.dist[shard] = p.dists;
+	in.cnt[shard] = p.counts;
+}
+
 extern "C" size_t pgemb_packed_topk_bytes(size_t nq, size_t k) { return nq * k * 12 + nq * 4; }
 
 extern "C" pgemb_status pgemb_merge_topk_packed_device(size_t nq, size_t n_shards, size_t k, const void *d_packed, size_t shard_stride_bytes,
@@ -2159,13 +2162,7 @@ extern "C" pgemb_status pgemb_merge_topk_packed_device(size_t nq, size_t n_shard
 	if (shard_stride_bytes < pgemb_packed_topk_bytes(nq, k) || (shard_stride_bytes & 7)) return fail(PGEMB_ERR_ARG, "bad shard stride");
 	ShardLists in;
 	memset(&in, 0, sizeof(in));
-	for (size_t s = 0; s < n_shards; s++)
-	{
-		const char *b = (const char *) d_packed + s * shard_stride_bytes;
-		in.lab[s] = (const uint64_t *) b;
-		in.dist[s] = (const float *) (b + nq * k * 8);
-		in.cnt[s] = (const int32_t *) (b + nq * k * 12);
-	}
+	for (size_t s = 0; s < n_shards; s++) set_shard(in, s, (const char *) d_packed + s * shard_stride_bytes, nq, k);
 	return launch_merge(nq, n_shards, k, in, nullptr, 0, 0, d_dists_out, d_labels_out, d_n_out, nullptr, (cudaStream_t) stream);
 }
 
@@ -2310,22 +2307,25 @@ extern "C" pgemb_status pgemb_exchange_attach(pgemb_exchange *ex, const void *ha
 	return PGEMB_OK;
 }
 
-extern "C" pgemb_status pgemb_sharded_search_device(pgemb_index *idx, pgemb_exchange *ex, size_t nq, const coord_t *d_queries, size_t ef, void *stream)
+// the result area of step `seq` in `buf` (this rank's buffer or a peer's): the step's parity picks one of the two
+static char *step_area(const pgemb_exchange *ex, char *buf, uint32_t seq) { return buf + (size_t) (seq & 1u) * ex->area_bytes; }
+
+// arguments of a local step; `k_name` is what the entry point calls its k
+static pgemb_status check_local_step(const pgemb_index *idx, const pgemb_exchange *ex, size_t nq, size_t k, const char *k_name)
 {
 	if (!idx || !ex) return fail(PGEMB_ERR_ARG, "null argument");
 	if (ex->world > 1 && !ex->attached) return fail(PGEMB_ERR_STATE, "pgemb_exchange_attach has not been called");
-	if (ef != ex->k) return fail(PGEMB_ERR_ARG, "ef differs from the exchange's k");
+	if (k != ex->k) return fail(PGEMB_ERR_ARG, std::string(k_name) + " differs from the exchange's k");
 	if (nq == 0 || nq > ex->max_nq) return fail(PGEMB_ERR_ARG, "nq out of range for this exchange");
 	if (idx->device != ex->device) return fail(PGEMB_ERR_ARG, "index and exchange live on different devices");
-	cudaStream_t s = (cudaStream_t) stream;
+	return PGEMB_OK;
+}
+
+// The local step has been enqueued: advance the sequence number and store it into every peer's flag array, after the step in
+// stream order.
+static pgemb_status publish_step(pgemb_exchange *ex, cudaStream_t s)
+{
 	ex->seq += 1;
-	char	 *area = ex->d_buf + (size_t) (ex->seq & 1u) * ex->area_bytes;
-	uint64_t *d_l = (uint64_t *) area;
-	float	 *d_d = (float *) (area + nq * ex->k * 8);
-	int32_t	 *d_n = (int32_t *) (area + nq * ex->k * 12);
-	pgemb_status st = launch_search(idx, nq, d_queries, (uint32_t) idx->meta.dim, nullptr, (uint32_t) idx->n, ef, 0, d_l, d_d, nullptr, d_n, nullptr, s, true);
-	if (st) return st;
-	// publish: my sequence number into every peer's flag array, after the search in stream order
 	uint32_t *src = &ex->h_seq[ex->seq & 63u];
 	*src = ex->seq;
 	for (int r = 0; r < ex->world; r++)
@@ -2336,29 +2336,27 @@ extern "C" pgemb_status pgemb_sharded_search_device(pgemb_index *idx, pgemb_exch
 	return PGEMB_OK;
 }
 
+extern "C" pgemb_status pgemb_sharded_search_device(pgemb_index *idx, pgemb_exchange *ex, size_t nq, const coord_t *d_queries, size_t ef, void *stream)
+{
+	pgemb_status st = check_local_step(idx, ex, nq, ef, "ef");
+	if (st) return st;
+	const PackedTopk out = packed_topk(step_area(ex, ex->d_buf, ex->seq + 1), nq, ex->k);
+	st = launch_search(idx, nq, d_queries, (uint32_t) idx->meta.dim, nullptr, (uint32_t) idx->n, ef, 0, out.labels, out.dists, nullptr, out.counts, nullptr,
+					   (cudaStream_t) stream, true);
+	if (st) return st;
+	return publish_step(ex, (cudaStream_t) stream);
+}
+
 // The brute-force scan as the local step of a sharded exchange (BASELINE configs[4]: every rank scans its id range for the whole
 // query batch): results land in this rank's result area, then the step is published to the peers exactly as a traversal's is.
 extern "C" pgemb_status pgemb_sharded_scan_device(pgemb_index *idx, pgemb_exchange *ex, size_t nq, const coord_t *d_queries, size_t k, void *stream)
 {
-	if (!idx || !ex) return fail(PGEMB_ERR_ARG, "null argument");
-	if (ex->world > 1 && !ex->attached) return fail(PGEMB_ERR_STATE, "pgemb_exchange_attach has not been called");
-	if (k != ex->k) return fail(PGEMB_ERR_ARG, "k differs from the exchange's k");
-	if (nq == 0 || nq > ex->max_nq) return fail(PGEMB_ERR_ARG, "nq out of range for this exchange");
-	if (idx->device != ex->device) return fail(PGEMB_ERR_ARG, "index and exchange live on different devices");
-	cudaStream_t s = (cudaStream_t) stream;
-	const uint32_t seq = ex->seq + 1;
-	char		  *area = ex->d_buf + (size_t) (seq & 1u) * ex->area_bytes;
-	pgemb_status   st = pgemb_scan_topk_device(idx, nq, d_queries, k, (label_t *) area, (dist_t *) (area + nq * ex->k * 8), (int32_t *) (area + nq * ex->k * 12), stream);
+	pgemb_status st = check_local_step(idx, ex, nq, k, "k");
 	if (st) return st;
-	ex->seq = seq;
-	uint32_t *src = &ex->h_seq[ex->seq & 63u];
-	*src = ex->seq;
-	for (int r = 0; r < ex->world; r++)
-	{
-		if (r == ex->rank) continue;
-		CU_TRY(cudaMemcpyAsync(ex->peer[r] + ex->off_flags + (size_t) ex->rank * 4, src, 4, cudaMemcpyHostToDevice, s));
-	}
-	return PGEMB_OK;
+	const PackedTopk out = packed_topk(step_area(ex, ex->d_buf, ex->seq + 1), nq, ex->k);
+	st = pgemb_scan_topk_device(idx, nq, d_queries, k, out.labels, out.dists, out.counts, stream);
+	if (st) return st;
+	return publish_step(ex, (cudaStream_t) stream);
 }
 
 extern "C" pgemb_status pgemb_sharded_merge_device(pgemb_exchange *ex, size_t nq, label_t *d_labels_out, dist_t *d_dists_out, int32_t *d_n_out, void *stream)
@@ -2370,13 +2368,7 @@ extern "C" pgemb_status pgemb_sharded_merge_device(pgemb_exchange *ex, size_t nq
 	cudaStream_t s = (cudaStream_t) stream;
 	ShardLists	 in;
 	memset(&in, 0, sizeof(in));
-	for (int r = 0; r < ex->world; r++)
-	{
-		const char *area = ex->peer[r] + (size_t) (ex->seq & 1u) * ex->area_bytes;
-		in.lab[r] = (const uint64_t *) area;
-		in.dist[r] = (const float *) (area + nq * ex->k * 8);
-		in.cnt[r] = (const int32_t *) (area + nq * ex->k * 12);
-	}
+	for (int r = 0; r < ex->world; r++) set_shard(in, (size_t) r, step_area(ex, ex->peer[r], ex->seq), nq, ex->k);
 	CU_TRY(cudaEventRecord(ex->ev0, s));
 	pgemb_status st = launch_merge(nq, (size_t) ex->world, ex->k, in, ex->world > 1 ? (const uint32_t *) (ex->d_buf + ex->off_flags) : nullptr, ex->seq,
 								   (uint32_t) ex->rank, d_dists_out, d_labels_out, d_n_out, ex->d_error, s);

@@ -160,6 +160,13 @@ def test_error_paths(pg):
         idx.links(2, 5)                                   # range beyond the index
     with pytest.raises(Exception):
         pg.HnswIndex(0, 2, 4, 4, "l2", capacity=3)        # dims must be given (embedding.c:219-221)
+    from pg_embedding_b200 import _lib
+    lib = _lib.load()
+    meta = _lib.HnswMetadata()
+    _lib.check(lib.pgemb_meta_init(C.byref(meta), 4, 2, 4, 4, 0))
+    meta.dist_func = 3                                    # no such metric: rejected before any path can dispatch on it
+    dev = C.c_void_p()
+    assert lib.pgemb_index_create(C.byref(meta), 3, 0, C.byref(dev)) == 2 and not dev.value
     idx.close()
 
 
