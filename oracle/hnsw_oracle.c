@@ -624,3 +624,37 @@ oracle_search_ids(HnswMetadata *meta, const coord_t *point, size_t ef, idx_t *id
 	heap_free(&top);
 	return (long) n;
 }
+
+/* Extension for tests: one batch of pgemb_build_bulk (include/pgemb_b200.h) on the stored, unbound nodes
+ * [first, first+n), stated with the primitives above.  Every member runs bindPoint's search against the graph
+ * as it was when the batch started; then each member, in id order, runs mutuallyConnectNewElement on its own
+ * search result.  This is the CUDA batch exactly: the members' link lists are blank and no stored list names
+ * them, so no search of the batch can reach one, and no member is ever a back-link target.  Hence a member's
+ * own list depends only on its search and on vectors, and every target takes its back-links in source-id
+ * order -- the order here.  Node 0 is skipped (hnswalg.cpp:227-228).  Returns 0, or -2 where the reference
+ * would throw. */
+int
+oracle_bind_batch(HnswMetadata *meta, idx_t first, size_t n)
+{
+	Heap *tops = (Heap *) calloc(n ? n : 1, sizeof(Heap));
+	bool  ok = true;
+
+	for (size_t i = 0; i < n; i++)
+	{
+		coord_t *pc;
+
+		if (first + i == 0)
+			continue;
+		hnsw_begin_read(meta, (idx_t) (first + i), NULL, &pc, NULL);
+		tops[i] = search_base_layer(meta, pc, meta->efConstruction);
+		hnsw_end_read(meta);
+	}
+	for (size_t i = 0; i < n; i++)
+	{
+		if (first + i != 0)
+			ok = connect_new_element(meta, NULL, (idx_t) (first + i), &tops[i]) && ok;
+		heap_free(&tops[i]);
+	}
+	free(tops);
+	return ok ? 0 : -2;
+}

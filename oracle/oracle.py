@@ -117,6 +117,8 @@ def load(which: str) -> C.CDLL:
         lib.oracle_cosine_from_parts.argtypes = [f32p, f32p, sz]
         lib.oracle_search_ids.restype = C.c_long
         lib.oracle_search_ids.argtypes = [vp, f32p, sz, u32p, f32p]
+        lib.oracle_bind_batch.restype = C.c_int
+        lib.oracle_bind_batch.argtypes = [vp, C.c_uint32, sz]
     _LIBS[which] = lib
     return lib
 
@@ -141,6 +143,21 @@ def dist_many(which: str, metric, a, b) -> np.ndarray:
     n, dim = b.shape
     out = np.empty(n, dtype=np.float32)
     lib.flat_dist_many(_metric(metric), _f32p(a), _f32p(b), dim, n, int(a.ndim == 1), _f32p(out))
+    return out
+
+
+def bulk_schedule(first: int, n: int, batch_max: int) -> list:
+    """pgemb_build_bulk's batches (capi.cu) over nodes [first, first+n) as (first node, size) pairs: a batch is at most 1/32 of
+    the nodes before it (at least 1), at most batch_max (clamped to [1, 65536]) and never runs past the end; node 0 is skipped."""
+    batch_max = min(max(int(batch_max), 1), 1 << 16)
+    pos, end, out = int(first), int(first) + int(n), []
+    while pos < end:
+        if pos == 0:
+            pos = 1             # node 0 has nothing to connect to
+            continue
+        b = min(max(pos // 32, 1), batch_max, end - pos)
+        out.append((pos, b))
+        pos += b
     return out
 
 
@@ -228,6 +245,18 @@ class FlatIndex:
         rc = self.lib.flat_bind(self.h, int(idx))
         if rc != 0:
             raise RuntimeError(f"bind failed rc={rc}")
+
+    def build_bulk(self, first: int, n: int, batch_max: int = 4096) -> list:
+        """(port only) pgemb_build_bulk's result on the stored, unbound nodes [first, first+n): its batch schedule (capi.cu) with
+        every batch bound by oracle_bind_batch.  Returns the batch sizes in order."""
+        if self.which != "port":
+            raise ValueError("build_bulk is a model stated with the C restatement's primitives: port only")
+        sizes = []
+        for pos, b in bulk_schedule(first, n, batch_max):
+            if self.lib.oracle_bind_batch(self.h, pos, b) != 0:
+                raise RuntimeError(f"bind batch [{pos}, {pos + b}) failed")
+            sizes.append(b)
+        return sizes
 
     def links(self, first: int = 0, n: int | None = None) -> np.ndarray:
         n = len(self) - first if n is None else n

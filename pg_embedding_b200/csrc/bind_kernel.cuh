@@ -9,7 +9,8 @@
 //         at NN = maxM and rewrite it farthest first (:182-222)
 //                                                       -> backlink_kernel (one CTA per (target) list)
 //
-// Exactness notes (checked bit-for-bit against the compiled reference in tests/test_gpu_bind.py):
+// Exactness notes (link lists checked byte for byte against the oracle: sequential binds in tests/test_gpu_parity.py, the
+// batched bulk build against the oracle's batch model in tests/test_gpu_bulk_build.py):
 //  * heuristic scan order = ascending distance to the base point, equal distances by DESCENDING id
 //    (resultSet holds pair(-dist,id), :126,:133); a candidate is kept iff no already kept r has
 //    dist(r,c) < dist(c,base) (:141-147, the early `break` only skips work); stop at NN kept (:131).

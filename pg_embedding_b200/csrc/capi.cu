@@ -1849,7 +1849,9 @@ static pgemb_status launch_backlinks(pgemb_index *idx, size_t count, cudaStream_
 	const GraphView g = graph_view(idx);
 	const size_t	maxM1 = idx->meta.maxM + 1;
 	const size_t	bl_smem = maxM1 * 8 * 2 + (idx->meta.maxM ? idx->meta.maxM : 1) * 8 + maxM1 * 4;
-	const uint32_t	n_pairs = (uint32_t) (count * (idx->meta.M ? idx->meta.M : 1));
+	// m = 0: no node selects a neighbour, so select_kernel wrote no pair slot -- not even a "none" marker -- and there is nothing to apply
+	if (idx->meta.M == 0) return PGEMB_OK;
+	const uint32_t	n_pairs = (uint32_t) (count * idx->meta.M);
 	const uint64_t *sorted = w.d_pairs;
 	if (count > 1)
 	{
@@ -2054,7 +2056,8 @@ extern "C" pgemb_status pgemb_build_exact(pgemb_index *idx, size_t first, size_t
 		st = launch_select(idx, w.d_qids, B, efc, false, s);
 		if (st) return st;
 		const uint32_t n_pairs_all = (uint32_t) (B * M);
-		if (B > 1)
+		// m = 0: no back-links, so no search of the batch can conflict with an earlier insert (and no pair slot was written)
+		if (B > 1 && idx->meta.M > 0)
 		{
 			uint32_t hfirst = (uint32_t) B;
 			CU_TRY(cudaMemcpyAsync(w.d_first, &hfirst, 4, cudaMemcpyHostToDevice, s));

@@ -113,31 +113,47 @@ def test_exact_parallel_build_orchestration(pg, oracle_mod):
         idx.close()
 
 
-def test_bulk_build_orchestration(pg, oracle_mod):
-    """pgemb_build_bulk: batch_max = 1 is the sequential build; larger batches give a valid graph (sorted back-link pairs,
-    per-target serialisation) that the traversal searches with the reference's results on that same graph."""
-    rng = np.random.default_rng(6)
-    dims, m, efc, n = 8, 4, 16, 400
-    x = rng.standard_normal((n, dims)).astype(np.float32)
-    orc = oracle_mod.FlatIndex("port", dims, m, efc, 64, "l2", capacity=n)
-    orc.build(x)
-    a = pg.HnswIndex(dims, m, efc, 64, "l2", capacity=n)
-    a.build(x, batch_max=1)
-    assert a.links().tobytes() == orc.links().tobytes()
-    a.close()
-    b = pg.HnswIndex(dims, m, efc, 64, "l2", capacity=n)
-    b.build(x, batch_max=32)
-    links = b.links()
-    cnt = links[:, 0]
-    assert cnt.max() <= 2 * m and (cnt[1:] > 0).all()
-    for i in range(n):
-        ids = links[i, 1:1 + cnt[i]]
-        assert (ids < n).all() and (ids != i).all() and len(set(ids.tolist())) == len(ids)
-    chk = oracle_mod.FlatIndex("port", dims, m, efc, 64, "l2", capacity=n)
-    chk.load_graph(x, links, b.labels())
-    q = rng.standard_normal((20, dims)).astype(np.float32)
-    assert b.search_batch(q, 10)["labels"].tobytes() == chk.search_many(q, 10)["labels"].tobytes()
-    b.close()
+@pytest.fixture(scope="module")
+def BB():
+    import test_gpu_bulk_build as bb     # GPU tests of the bulk build against the oracle's batch model: bodies reused below
+    return bb
+
+
+def test_bulk_build_orchestration(pg, BB, oracle_mod):
+    """pgemb_build_bulk equals the oracle's batch model byte for byte at batch_max 1 (one node per batch, pairs unsorted), 8
+    (the staged select) and 64 (batches of up to 15 here: the unstaged select and the sorted pairs), and its graph searches
+    like the oracle's.  L2 8-d and the tie-heavy 3-d grid."""
+    for cfg in BB.EMU_CASES[:2]:
+        for bmax in (1, 8, 64):
+            sizes = BB.check_bulk_build(pg, oracle_mod, cfg, bmax, efs=(10,))
+            assert max(sizes) == bmax if bmax <= 8 else 8 < max(sizes) < bmax, (cfg[0], bmax, max(sizes))
+
+
+@pytest.mark.parametrize("ci", [2, 3, 4], ids=["cosine-d12", "m0", "m1"])
+def test_bulk_build_metrics_and_degrees(pg, BB, oracle_mod, ci):
+    """Cosine, and m = 0 (no pair slot is written: the back-link step must read none it did not mark) and m = 1, in bulk
+    builds and in sequential inserts followed by one."""
+    for bmax in (1, 64):
+        BB.check_bulk_build(pg, oracle_mod, BB.EMU_CASES[ci], bmax, efs=(10,))
+    BB.check_bulk_build(pg, oracle_mod, BB.EMU_CASES[ci], 64, plan="insert", efs=(10,))
+
+
+def test_edge_parameters_m0(pg, G, oracle_mod):
+    """m = 0 through insert_many and the exact parallel build: the emulated runtime fills fresh allocations with 0xCD, so a
+    pair slot read before it is written names a node far beyond the index."""
+    G.test_edge_parameters(pg, oracle_mod, G.EDGE_CFGS[1])
+    G.test_exact_parallel_build_equals_sequential(pg, oracle_mod, G.EXACT_CFGS[-1])
+
+
+@pytest.mark.parametrize("plan", ["two", "reserve", "insert"])
+def test_bulk_build_incremental(pg, BB, oracle_mod, plan):
+    BB.check_bulk_build(pg, oracle_mod, BB.EMU_CASES[0], 64, plan=plan, efs=(10,))
+
+
+@pytest.mark.parametrize("coop", ["0", "1"])
+def test_bulk_build_kernel_modes(pg, BB, oracle_mod, coop):
+    """Two emulated SMs: with PGEMB_COOP=1 batches of one or two nodes search in latency mode, larger ones in throughput mode."""
+    BB.check_bulk_build(pg, oracle_mod, BB.EMU_CASES[0], 64, coop=coop, efs=(10,))
 
 
 def test_index_grows_in_place(pg, G, oracle_mod):

@@ -509,6 +509,7 @@ EXACT_CFGS = [
     (32, 8, 64, 6000, dict(), "l2"),
     (128, 16, 100, 4000, dict(), "manhattan"),
     (768, 32, 200, 1500, dict(), "cosine"),
+    (5, 0, 8, 300, dict(), "manhattan"),              # m=0: no back-links, so nothing to validate
 ]
 
 
