@@ -122,8 +122,8 @@ __global__ void scan_dist_kernel(const float *__restrict__ vectors, const float 
 	if (pair < total && sub == 0) out[pair] = d;
 }
 
-// Device-pointer epilogue of the brute-force scan (pgemb_scan_topk_device): the running top-k (order keys, labels, counts) in
-// the caller's layout -- distances as floats, unused tail = (~0, +inf) -- exactly what the host epilogue of pgemb_scan_topk writes.
+// Epilogue of the brute-force scan (both entry points; the host-pointer one copies its output back): the running top-k (order
+// keys, labels, counts) in the caller's layout -- distances as floats, unused tail = (~0, +inf).
 __global__ void scan_finish_kernel(const uint32_t *__restrict__ top_d, const uint64_t *__restrict__ top_l, const uint32_t *__restrict__ top_n, uint32_t nq,
 								   uint32_t k, uint64_t *__restrict__ labels_out, float *__restrict__ dists_out, int32_t *__restrict__ n_out)
 {

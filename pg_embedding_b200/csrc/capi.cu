@@ -8,7 +8,6 @@
 // entry point fails with PGEMB_ERR_CUDA.
 #include <algorithm>
 #include <atomic>
-#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -137,7 +136,7 @@ struct pgemb_index
 	uint32_t	 *d_visited = nullptr, *d_vlog = nullptr, *d_vhash = nullptr;
 	uint32_t	  ws_vh = 0;  // allocated hash entries per slot
 	size_t		  l2_persist_max = 0, l2_window_max = 0;
-	bool		  l2_limit_dropped = false;	 // the scan path gave the persisting-L2 set-aside back (scan_topk_impl)
+	bool		  l2_limit_dropped = false;	 // the scan path gave the persisting-L2 set-aside back (scan_filter_pass)
 	// link lists that came from the caller have not been checked for repeated ids yet / result of the last check
 	bool links_checked = true, links_distinct = true;
 	uint64_t	 *d_ovf = nullptr;
@@ -1253,29 +1252,217 @@ static pgemb_status launch_scan_filter(pgemb_index *idx, int metric, const float
 #endif
 }
 
-static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
-								   int32_t *n_out, bool allow_tc, bool *tc_violation, bool device_io);
-static pgemb_status scan_topk_groups(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out, int32_t *n_out,
-									 bool device_io);
-
-extern "C" pgemb_status pgemb_scan_topk(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
-										int32_t *n_out)
+// Every decision of one scan call, from the index, the batch and the PGEMB_SCAN_* knobs.  The knobs are read on every call,
+// so that a caller can switch them between calls.
+struct ScanPlan
 {
-	return scan_topk_groups(idx, nq, queries, k, labels_out, dists_out, n_out, false);
+	bool   tc;			  // tensor-core filter + exact re-scoring; else the exact kernels alone
+	bool   tiled;		  // exact pass: scan_tile_kernel (same bits as scan_dist_kernel, rows read once per query tile)
+	int	   l2reset;		  // filter pass: what to give back of a traversal's L2 persistence window (scan_filter_pass)
+	float  rel;			  // filter pass: error bound relative to |q||v|
+	size_t chunk;		  // exact pass: rows per distance / select launch pair
+	size_t c0, cap;		  // filter pass: first chunk (every row of it is a candidate), candidate list length per query
+	size_t growth, cmax;  // filter pass: chunk growth factor, largest chunk
+};
+
+static ScanPlan plan_scan(const pgemb_index *idx, size_t nq, size_t k, bool allow_tc)
+{
+	ScanPlan p;
+	// PGEMB_SCAN_TC: 0 = exact kernels only, 1 (default) = tensor-core filter for L2 / cosine when the table has at least
+	// PGEMB_SCAN_TC_MIN_ROWS (default 4096) rows, 2 = always (tests).
+	const int mode = env_int("PGEMB_SCAN_TC", 1);
+	p.tc = allow_tc && idx->meta.dist_func != DIST_MANHATTAN && mode > 0 && (mode >= 2 || idx->n >= (size_t) env_int("PGEMB_SCAN_TC_MIN_ROWS", 4096));
+	p.tiled = env_int("PGEMB_SCAN_TILED", 1) != 0;
+	// PGEMB_SCAN_L2RESET: 0 = leave as is, 1 = reset lines + window, 2 (default) = also drop the set-aside limit until the next
+	// traversal configures it again
+	p.l2reset = env_int("PGEMB_SCAN_L2RESET", 2);
+	p.rel = scan_tc_rel(idx->meta.dim);
+	int lg = env_int("PGEMB_SCAN_CHUNK_LOG2", 0);
+	p.chunk = (lg >= 8 && lg <= 20) ? (size_t) 1 << lg : (size_t) 1 << 14;
+	while (p.chunk > 256 && nq * p.chunk * 4 > ((size_t) 256 << 20)) p.chunk >>= 1;
+	// tensor-core path: first chunk establishes the threshold (every row of it is a candidate), then x2 per chunk (PGEMB_SCAN_TC_GROWTH)
+	lg = env_int("PGEMB_SCAN_TC_CHUNK0_LOG2", 0);
+	p.c0 = (lg >= 5 && lg <= 20) ? (size_t) 1 << lg : ((2 * k > 256 ? 2 * k : 256) + 255) / 256 * 256;
+	const int cap = env_int("PGEMB_SCAN_TC_CAP", 0);
+	p.cap = cap > 0 ? (size_t) cap : (2 * p.c0 > 4096 ? 2 * p.c0 : 4096);
+	p.growth = (size_t) env_int("PGEMB_SCAN_TC_GROWTH", 2);	// measured (profiles/r2_call10_scan_growth_sweep.log): 2 / 3 / 4 / 8 -> 6.7 / 7.7 / 8.0 / 8.6 ms per 1024 x 1M x 768 scan at k 64
+	if (p.growth < 2) p.growth = 2;
+	// chunks stop growing at 2^20 rows (PGEMB_SCAN_TC_CHUNK_MAX_LOG2): the candidate lists are sized for what passes the filter in
+	// one chunk, and a table of tens of millions of rows must not end in one chunk of half the table
+	lg = env_int("PGEMB_SCAN_TC_CHUNK_MAX_LOG2", 0);
+	p.cmax = (lg >= 8 && lg <= 30) ? (size_t) 1 << lg : (size_t) 1 << 20;
+	return p;
 }
 
-// The same scan with DEVICE pointers in and out (the caller's stream is only synchronised with: the scan runs on the index's own
-// stream and has finished when the call returns).  For callers whose queries and results live in HBM already: the sharded scan.
-extern "C" pgemb_status pgemb_scan_topk_device(pgemb_index *idx, size_t nq, const coord_t *d_queries, size_t k, label_t *d_labels_out, dist_t *d_dists_out,
-											   int32_t *d_n_out, void *stream)
+// The arrays of one scan in the staging buffer.  q: [nq][row_f] queries; dist: [nq][chunk] distances of the exact pass;
+// td, tl, tn: running top-k (order keys, labels, counts); sd, sl: select / re-score scratch of the same shape; qn: query squared
+// norms; cn, qc, cr, cs: candidate counts, filter constants, candidate rows, candidate products; cnt: [0] re-scored,
+// [1] tripwire, [2] overflowed queries
+struct ScanBuffers
 {
-	if (idx && stream)
+	float	 *q = nullptr, *dist = nullptr, *qn = nullptr, *cs = nullptr;
+	uint32_t *td = nullptr, *sd = nullptr, *tn = nullptr, *cn = nullptr, *cr = nullptr, *cnt = nullptr;
+	uint64_t *tl = nullptr, *sl = nullptr;
+	float2	 *qc = nullptr;
+};
+
+// nq queries into d_q at row_f stride, zero padded (the TMA tensor map reads whole 16-byte units)
+static pgemb_status stage_queries(const pgemb_index *idx, float *d_q, const coord_t *queries, size_t nq, cudaMemcpyKind kind, cudaStream_t s)
+{
+	const size_t rf = idx->row_f, dim = idx->meta.dim;
+	if (rf != dim) CU_TRY(cudaMemsetAsync(d_q, 0, nq * rf * 4, s));
+	CU_TRY(cudaMemcpy2DAsync(d_q, rf * 4, queries, dim * 4, dim * 4, nq, kind, s));
+	return PGEMB_OK;
+}
+
+// K6: tensor-core filter + exact re-scoring over the whole table in geometrically growing chunks (scan_umma_kernel.cuh)
+static pgemb_status scan_filter_pass(pgemb_index *idx, const ScanPlan &p, const ScanBuffers &b, size_t nq, size_t k, cudaStream_t s)
+{
+	// The filter lives on L2 reuse (the table streams from HBM once, the other query tiles re-read it from L2).  A traversal
+	// on this index leaves an L2 persistence window behind (the per-slot visited sets, launch_search): give those lines and
+	// the set-aside back before scanning.
+	if (p.l2reset > 0 && idx->last_l2_base != nullptr)
 	{
-		pgemb_status st = set_device(idx);
-		if (st) return st;
-		CU_TRY(cudaStreamSynchronize((cudaStream_t) stream));  // the queries may have been produced on it
+		cudaStreamAttrValue av;
+		memset(&av, 0, sizeof(av));
+		av.accessPolicyWindow.num_bytes = 0;
+		if (cudaStreamSetAttribute(idx->last_l2_stream ? idx->last_l2_stream : s, cudaStreamAttributeAccessPolicyWindow, &av) != cudaSuccess) cudaGetLastError();
+		if (cudaCtxResetPersistingL2Cache() != cudaSuccess) cudaGetLastError();
+		if (p.l2reset > 1 && cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, 0) != cudaSuccess) cudaGetLastError();
+		idx->last_l2_base = nullptr;
+		idx->l2_limit_dropped = p.l2reset > 1;
 	}
-	return scan_topk_groups(idx, nq, d_queries, k, d_labels_out, d_dists_out, d_n_out, true);
+	pgemb_status st = ensure_row_norms(idx, s);
+	if (st) return st;
+	const int	 metric = (int) idx->meta.dist_func;
+	const size_t N = idx->n, dim = idx->meta.dim, rf = idx->row_f;
+	CU_TRY(cudaMemsetAsync(b.cnt, 0, 16, s));
+	st = with_tc_metric(metric, [&](auto m) -> pgemb_status {
+		PGEMB_LAUNCH(scan_qconst_init_kernel<decltype(m)::value>, (uint32_t) ((nq + 127) / 128), 128, 0, s, b.qn, (uint32_t) nq, p.rel, b.qc, b.cn);
+		return PGEMB_OK;
+	});
+	if (st) return st;
+	g_launches++;
+	size_t csize = p.c0;
+	for (size_t r0 = 0; r0 < N;)
+	{
+		size_t nr = N - r0 < csize ? N - r0 : csize;
+		if (N - r0 - nr < nr / 8) nr = N - r0;	// do not leave a sliver for an extra launch pair
+		st = launch_scan_filter(idx, metric, b.q, b.qn, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, p.rel, b.qc, b.cr, b.cs, b.cn, (uint32_t) p.cap, nullptr, s);
+		if (st) return st;
+		st = with_tc_metric(metric, [&](auto m) -> pgemb_status {
+			PGEMB_LAUNCH(scan_rescore_kernel<decltype(m)::value>, (uint32_t) nq, 128, 0, s, idx->d_vectors, idx->row_f, (uint32_t) dim, idx->d_norms, b.q,
+						 (uint32_t) rf, b.qn, idx->d_labels, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, (uint32_t) k, p.rel, b.cr, b.cs, b.cn, (uint32_t) p.cap,
+						 b.td, b.tl, b.tn, b.sd, b.sl, b.qc, b.cnt);
+			return PGEMB_OK;
+		});
+		if (st) return st;
+		g_launches++;
+		CU_TRY(cudaGetLastError());
+		r0 += nr;
+		csize *= p.growth;
+		if (csize > p.cmax) csize = p.cmax > p.c0 ? p.cmax : p.c0;
+	}
+	g_scan_tc++;
+	g_scan_pairs += (uint64_t) nq * N;
+	return PGEMB_OK;
+}
+
+// the exact kernels: per chunk of rows, every (query, row) distance, then its fold into the running top-k
+static pgemb_status scan_exact_pass(pgemb_index *idx, const ScanPlan &p, const ScanBuffers &b, size_t nq, size_t k, cudaStream_t s)
+{
+	const int	   metric = (int) idx->meta.dist_func;
+	const size_t   N = idx->n, dim = idx->meta.dim, rf = idx->row_f;
+	const uint32_t lanes = (metric == DIST_L2) ? 8 : 4;
+	g_scan_exact++;
+	for (size_t r0 = 0; r0 < N; r0 += p.chunk)
+	{
+		const size_t   nr = (N - r0 < p.chunk) ? (N - r0) : p.chunk;
+		const uint32_t threads = 128;
+		const uint32_t blocks = (uint32_t) ((nq * nr * lanes + threads - 1) / threads);
+		const pgemb_status st = with_metric(metric, [&](auto m) -> pgemb_status {
+			constexpr uint32_t tq = ScanTile<decltype(m)::value>::TQ;
+			if (p.tiled)
+				PGEMB_LAUNCH(scan_tile_kernel<decltype(m)::value>, dim3((uint32_t) ((nq + tq - 1) / tq), (uint32_t) ((nr + kScanTileRows - 1) / kScanTileRows)),
+							 kScanThreads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim, b.q, (uint32_t) rf, b.qn, (uint32_t) nq,
+							 (uint32_t) r0, (uint32_t) nr, b.dist);
+			else
+				PGEMB_LAUNCH(scan_dist_kernel<decltype(m)::value>, blocks, threads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim, b.q,
+							 (uint32_t) rf, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, b.dist);
+			return PGEMB_OK;
+		});
+		if (st) return st;
+		PGEMB_LAUNCH(scan_select_kernel, (uint32_t) ((nq + 3) / 4), 128, 0, s, b.dist, idx->d_labels, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, (uint32_t) k,
+					 b.td, b.tl, b.tn, b.sd, b.sl);
+		g_launches += 2;
+		CU_TRY(cudaGetLastError());
+	}
+	return PGEMB_OK;
+}
+
+// The results in the caller's layout (scan_finish_kernel), then the tripwire counters into cnt[4] if asked for, and one
+// synchronisation.  Device pointers receive the results directly.  For host pointers the kernel writes into the select /
+// re-score scratch and the candidate counts, which have the outputs' shapes and are dead after the last pass, and the
+// results are copied from there.
+static pgemb_status scan_hand_off(const ScanBuffers &b, size_t nq, size_t k, label_t *labels_out, dist_t *dists_out, int32_t *n_out, bool device_io,
+								  uint32_t *cnt, cudaStream_t s)
+{
+	label_t *lo = device_io ? labels_out : b.sl;
+	dist_t	*dout = (device_io || !dists_out) ? dists_out : (dist_t *) b.sd;
+	int32_t *no = device_io ? n_out : (int32_t *) b.cn;
+	PGEMB_LAUNCH(scan_finish_kernel, (uint32_t) ((nq * k + 255) / 256), 256, 0, s, b.td, b.tl, b.tn, (uint32_t) nq, (uint32_t) k, lo, dout, no);
+	g_launches++;
+	CU_TRY(cudaGetLastError());
+	if (!device_io)
+	{
+		CU_TRY(cudaMemcpyAsync(labels_out, lo, nq * k * 8, cudaMemcpyDeviceToHost, s));
+		if (dists_out) CU_TRY(cudaMemcpyAsync(dists_out, dout, nq * k * 4, cudaMemcpyDeviceToHost, s));
+		CU_TRY(cudaMemcpyAsync(n_out, no, nq * 4, cudaMemcpyDeviceToHost, s));
+	}
+	if (cnt) CU_TRY(cudaMemcpyAsync(cnt, b.cnt, 16, cudaMemcpyDeviceToHost, s));
+	CU_TRY(cudaStreamSynchronize(s));
+	return PGEMB_OK;
+}
+
+// One group of queries: stage them, run one pass over the table, hand the results over.  *tc_violation: the tensor-core
+// filter saw a product outside its assumed error bound.
+static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
+								   int32_t *n_out, bool allow_tc, bool *tc_violation, bool device_io)
+{
+	*tc_violation = false;
+	pgemb_status st = set_device(idx);
+	if (st) return st;
+	const ScanPlan p = plan_scan(idx, nq, k, allow_tc);
+	cudaStream_t   s = idx->stream;
+	const size_t   qb = nq * idx->row_f * 4, db = p.tc ? 0 : nq * p.chunk * 4, kd = nq * k * 4, kl = nq * k * 8, nb = nq * 4;
+	const size_t   cb = p.tc ? nq * p.cap * 4 : 0;
+	ScanBuffers	   b;
+	const StageLayout stage{{b.q, qb}, {b.dist, db}, {b.td, kd}, {b.sd, kd}, {b.tl, kl}, {b.sl, kl}, {b.tn, nb},
+							{b.qn, nb}, {b.cn, nb}, {b.qc, nq * 8}, {b.cr, cb}, {b.cs, cb}, {b.cnt, 16}};
+	st = ensure_stage(idx, stage.bytes + 256);
+	if (st) return st;
+	stage.place(idx->d_stage);
+	st = stage_queries(idx, b.q, queries, nq, device_io ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s);
+	if (st) return st;
+	CU_TRY(cudaMemsetAsync(b.tn, 0, nb, s));
+	if (p.tc || (p.tiled && idx->meta.dist_func == DIST_COSINE))
+	{
+		PGEMB_LAUNCH(norms_kernel, (uint32_t) ((nq * 4 + 127) / 128), 128, 0, s, b.q, idx->row_f, (uint32_t) idx->meta.dim, 0u, (uint32_t) nq, b.qn);
+		g_launches++;
+		CU_TRY(cudaGetLastError());
+	}
+	st = p.tc ? scan_filter_pass(idx, p, b, nq, k, s) : scan_exact_pass(idx, p, b, nq, k, s);
+	if (st) return st;
+	uint32_t cnt[4] = {0, 0, 0, 0};
+	st = scan_hand_off(b, nq, k, labels_out, dists_out, n_out, device_io, p.tc ? cnt : nullptr, s);
+	if (st) return st;
+	if (p.tc)
+	{
+		g_scan_rescored += cnt[0];
+		g_scan_overflow += cnt[2];
+		*tc_violation = cnt[1] != 0;
+	}
+	return PGEMB_OK;
 }
 
 static pgemb_status scan_topk_groups(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out, int32_t *n_out,
@@ -1306,225 +1493,24 @@ static pgemb_status scan_topk_groups(pgemb_index *idx, size_t nq, const coord_t 
 	return PGEMB_OK;
 }
 
-// PGEMB_SCAN_TC: 0 = exact kernels only, 1 (default) = tensor-core filter for L2 / cosine when the table has at least
-// PGEMB_SCAN_TC_MIN_ROWS (default 4096) rows, 2 = always (tests).
-static bool scan_use_tc(const pgemb_index *idx, bool allow_tc)
+extern "C" pgemb_status pgemb_scan_topk(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
+										int32_t *n_out)
 {
-	if (!allow_tc || idx->meta.dist_func == DIST_MANHATTAN) return false;
-	const int mode = env_int("PGEMB_SCAN_TC", 1);
-	if (mode <= 0) return false;
-	if (mode >= 2) return true;
-	return idx->n >= (size_t) env_int("PGEMB_SCAN_TC_MIN_ROWS", 4096);
+	return scan_topk_groups(idx, nq, queries, k, labels_out, dists_out, n_out, false);
 }
 
-static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
-								   int32_t *n_out, bool allow_tc, bool *tc_violation, bool device_io)
+// The same scan with DEVICE pointers in and out (the caller's stream is only synchronised with: the scan runs on the index's own
+// stream and has finished when the call returns).  For callers whose queries and results live in HBM already: the sharded scan.
+extern "C" pgemb_status pgemb_scan_topk_device(pgemb_index *idx, size_t nq, const coord_t *d_queries, size_t k, label_t *d_labels_out, dist_t *d_dists_out,
+											   int32_t *d_n_out, void *stream)
 {
-	*tc_violation = false;
-	pgemb_status st = set_device(idx);
-	if (st) return st;
-	// PGEMB_SCAN_TIMING=1: host-side time line of one scan on stderr (where does a call spend its time besides the kernels)
-	const bool timing = env_int("PGEMB_SCAN_TIMING", 0) != 0;
-	const auto t_begin = std::chrono::steady_clock::now();
-	auto	   since = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
-	double	   t_staged = 0, t_enqueued = 0, t_synced = 0;
-	const size_t dim = idx->meta.dim;
-	const size_t N = idx->n;
-	const size_t rf = idx->row_f;
-	const bool	 tc = scan_use_tc(idx, allow_tc);
-	const int	 metric = (int) idx->meta.dist_func;
-	cudaStream_t s = idx->stream;
-	// ---- staging ------------------------------------------------------------------------------------------------
-	size_t chunk = (size_t) 1 << 14;  // exact path: rows per distance / select launch pair
+	if (idx && stream)
 	{
-		const int lg = env_int("PGEMB_SCAN_CHUNK_LOG2", 0);
-		if (lg >= 8 && lg <= 20) chunk = (size_t) 1 << lg;
-	}
-	while (chunk > 256 && nq * chunk * 4 > ((size_t) 256 << 20)) chunk >>= 1;
-	// tensor-core path: first chunk establishes the threshold (every row of it is a candidate), then x2 per chunk (PGEMB_SCAN_TC_GROWTH)
-	size_t c0 = ((2 * k > 256 ? 2 * k : 256) + 255) / 256 * 256;
-	{
-		const int lg = env_int("PGEMB_SCAN_TC_CHUNK0_LOG2", 0);
-		if (lg >= 5 && lg <= 20) c0 = (size_t) 1 << lg;
-	}
-	size_t cap = 2 * c0 > 4096 ? 2 * c0 : 4096;
-	{
-		const int v = env_int("PGEMB_SCAN_TC_CAP", 0);
-		if (v > 0) cap = (size_t) v;
-	}
-	const size_t qb = nq * rf * 4, db = tc ? 0 : nq * chunk * 4, kd = nq * k * 4, kl = nq * k * 8, nb = nq * 4;
-	const size_t cb = tc ? nq * cap * 4 : 0;
-	float	 *d_q = nullptr, *d_dist = nullptr, *d_qn = nullptr, *d_cs = nullptr;
-	uint32_t *d_td = nullptr, *d_sd = nullptr, *d_tn = nullptr, *d_cn = nullptr, *d_cr = nullptr, *d_cnt = nullptr;
-	uint64_t *d_tl = nullptr, *d_sl = nullptr;
-	float2	 *d_qc = nullptr;
-	// d_q: [nq][row_f], zero padded (the TMA tensor map reads whole 16-byte units); d_cn, d_qc, d_cr, d_cs: candidate counts, filter
-	// constants, candidate rows, candidate products; d_cnt: [0] re-scored, [1] tripwire, [2] overflowed queries
-	const StageLayout stage{{d_q, qb}, {d_dist, db}, {d_td, kd}, {d_sd, kd}, {d_tl, kl}, {d_sl, kl}, {d_tn, nb},
-							{d_qn, nb}, {d_cn, nb}, {d_qc, nq * 8}, {d_cr, cb}, {d_cs, cb}, {d_cnt, 16}};
-	st = ensure_stage(idx, stage.bytes + 256);
-	if (st) return st;
-	stage.place(idx->d_stage);
-	if (rf != dim) CU_TRY(cudaMemsetAsync(d_q, 0, qb, s));
-	CU_TRY(cudaMemcpy2DAsync(d_q, rf * 4, queries, dim * 4, dim * 4, nq, device_io ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
-	CU_TRY(cudaMemsetAsync(d_tn, 0, nb, s));
-	if (timing)
-	{
-		cudaStreamSynchronize(s);
-		t_staged = since();
-	}
-	// tiled distance step (scan_tile_kernel.cuh): same bits as scan_dist_kernel, rows read once per query tile
-	const bool tiled = env_int("PGEMB_SCAN_TILED", 1) != 0;
-	if (tc || (tiled && metric == DIST_COSINE))
-	{
-		PGEMB_LAUNCH(norms_kernel, (uint32_t) ((nq * 4 + 127) / 128), 128, 0, s, d_q, (uint32_t) rf, (uint32_t) dim, 0u, (uint32_t) nq, d_qn);
-		g_launches++;
-		CU_TRY(cudaGetLastError());
-	}
-	if (tc)
-	{
-		// ---- K6: tensor-core filter + exact re-scoring, geometric chunks -----------------------------------------------
-		// The filter lives on L2 reuse (the table streams from HBM once, the other query tiles re-read it from L2).  A traversal
-		// on this index leaves an L2 persistence window behind (the per-slot visited sets, launch_search): give those lines and
-		// the set-aside back before scanning.  PGEMB_SCAN_L2RESET: 0 = leave as is, 1 = reset lines + window, 2 (default) = also
-		// drop the set-aside limit until the next traversal configures it again.
-		const int l2reset = env_int("PGEMB_SCAN_L2RESET", 2);
-		if (l2reset > 0 && idx->last_l2_base != nullptr)
-		{
-			cudaStreamAttrValue av;
-			memset(&av, 0, sizeof(av));
-			av.accessPolicyWindow.num_bytes = 0;
-			if (cudaStreamSetAttribute(idx->last_l2_stream ? idx->last_l2_stream : s, cudaStreamAttributeAccessPolicyWindow, &av) != cudaSuccess) cudaGetLastError();
-			if (cudaCtxResetPersistingL2Cache() != cudaSuccess) cudaGetLastError();
-			if (l2reset > 1 && cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, 0) != cudaSuccess) cudaGetLastError();
-			idx->last_l2_base = nullptr;
-			idx->l2_limit_dropped = l2reset > 1;
-		}
-		st = ensure_row_norms(idx, s);
+		pgemb_status st = set_device(idx);
 		if (st) return st;
-		const float rel = scan_tc_rel(dim);
-		CU_TRY(cudaMemsetAsync(d_cnt, 0, 16, s));
-		st = with_tc_metric(metric, [&](auto m) -> pgemb_status {
-			PGEMB_LAUNCH(scan_qconst_init_kernel<decltype(m)::value>, (uint32_t) ((nq + 127) / 128), 128, 0, s, d_qn, (uint32_t) nq, rel, d_qc, d_cn);
-			return PGEMB_OK;
-		});
-		if (st) return st;
-		g_launches++;
-		size_t csize = c0;
-		size_t growth = (size_t) env_int("PGEMB_SCAN_TC_GROWTH", 2);	// measured (profiles/r2_call10_scan_growth_sweep.log): 2 / 3 / 4 / 8 -> 6.7 / 7.7 / 8.0 / 8.6 ms per 1024 x 1M x 768 scan at k 64
-		if (growth < 2) growth = 2;
-		// chunks stop growing at 2^20 rows (PGEMB_SCAN_TC_CHUNK_MAX_LOG2): the candidate lists are sized for what passes the filter in
-		// one chunk, and a table of tens of millions of rows must not end in one chunk of half the table
-		size_t cmax = (size_t) 1 << 20;
-		{
-			const int lg = env_int("PGEMB_SCAN_TC_CHUNK_MAX_LOG2", 0);
-			if (lg >= 8 && lg <= 30) cmax = (size_t) 1 << lg;
-		}
-		for (size_t r0 = 0; r0 < N;)
-		{
-			size_t nr = N - r0 < csize ? N - r0 : csize;
-			if (N - r0 - nr < nr / 8) nr = N - r0;	// do not leave a sliver for an extra launch pair
-			st = launch_scan_filter(idx, metric, d_q, d_qn, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, rel, d_qc, d_cr, d_cs, d_cn, (uint32_t) cap, nullptr, s);
-			if (st) return st;
-			st = with_tc_metric(metric, [&](auto m) -> pgemb_status {
-				PGEMB_LAUNCH(scan_rescore_kernel<decltype(m)::value>, (uint32_t) nq, 128, 0, s, idx->d_vectors, idx->row_f, (uint32_t) dim, idx->d_norms, d_q,
-							 (uint32_t) rf, d_qn, idx->d_labels, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, (uint32_t) k, rel, d_cr, d_cs, d_cn, (uint32_t) cap,
-							 d_td, d_tl, d_tn, d_sd, d_sl, d_qc, d_cnt);
-				return PGEMB_OK;
-			});
-			if (st) return st;
-			g_launches++;
-			CU_TRY(cudaGetLastError());
-			r0 += nr;
-			csize *= growth;
-			if (csize > cmax) csize = cmax > c0 ? cmax : c0;
-		}
-		g_scan_tc++;
-		g_scan_pairs += (uint64_t) nq * N;
+		CU_TRY(cudaStreamSynchronize((cudaStream_t) stream));  // the queries may have been produced on it
 	}
-	else
-	{
-		g_scan_exact++;
-		const uint32_t lanes = (metric == DIST_L2) ? 8 : 4;
-		for (size_t r0 = 0; r0 < N; r0 += chunk)
-		{
-			const size_t   nr = (N - r0 < chunk) ? (N - r0) : chunk;
-			const uint32_t threads = 128;
-			const uint32_t blocks = (uint32_t) ((nq * nr * lanes + threads - 1) / threads);
-			st = with_metric(metric, [&](auto m) -> pgemb_status {
-				constexpr uint32_t tq = ScanTile<decltype(m)::value>::TQ;
-				if (tiled)
-					PGEMB_LAUNCH(scan_tile_kernel<decltype(m)::value>, dim3((uint32_t) ((nq + tq - 1) / tq), (uint32_t) ((nr + kScanTileRows - 1) / kScanTileRows)),
-								 kScanThreads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim, d_q, (uint32_t) rf, d_qn, (uint32_t) nq,
-								 (uint32_t) r0, (uint32_t) nr, d_dist);
-				else
-					PGEMB_LAUNCH(scan_dist_kernel<decltype(m)::value>, blocks, threads, 0, s, idx->d_vectors, idx->d_norms, idx->row_f, (uint32_t) dim, d_q,
-								 (uint32_t) rf, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, d_dist);
-				return PGEMB_OK;
-			});
-			if (st) return st;
-			PGEMB_LAUNCH(scan_select_kernel, (uint32_t) ((nq + 3) / 4), 128, 0, s, d_dist, idx->d_labels, (uint32_t) nq, (uint32_t) r0, (uint32_t) nr, (uint32_t) k,
-																		 d_td, d_tl, d_tn, d_sd, d_sl);
-			g_launches += 2;
-			CU_TRY(cudaGetLastError());
-		}
-	}
-	uint32_t cnt[4] = {0, 0, 0, 0};
-	if (device_io)
-	{
-		PGEMB_LAUNCH(scan_finish_kernel, (uint32_t) ((nq * k + 255) / 256), 256, 0, s, d_td, d_tl, d_tn, (uint32_t) nq, (uint32_t) k, labels_out, dists_out, n_out);
-		g_launches++;
-		CU_TRY(cudaGetLastError());
-		if (timing) t_enqueued = since();
-		if (tc) CU_TRY(cudaMemcpyAsync(cnt, d_cnt, 16, cudaMemcpyDeviceToHost, s));
-		CU_TRY(cudaStreamSynchronize(s));
-		if (timing) t_synced = since();
-	}
-	else
-	{
-		std::vector<uint32_t> hd, hn;
-		try
-		{
-			hd.resize(nq * k);
-			hn.resize(nq);
-		}
-		catch (const std::bad_alloc &)
-		{
-			cudaStreamSynchronize(s);
-			return fail(PGEMB_ERR_NOMEM, "out of host memory");  // no C++ exception crosses the C ABI
-		}
-		if (timing)
-		{
-			t_enqueued = since();
-			cudaStreamSynchronize(s);
-			t_synced = since();
-		}
-		CU_TRY(cudaMemcpyAsync(hd.data(), d_td, kd, cudaMemcpyDeviceToHost, s));
-		CU_TRY(cudaMemcpyAsync(labels_out, d_tl, kl, cudaMemcpyDeviceToHost, s));
-		CU_TRY(cudaMemcpyAsync(hn.data(), d_tn, nb, cudaMemcpyDeviceToHost, s));
-		if (tc) CU_TRY(cudaMemcpyAsync(cnt, d_cnt, 16, cudaMemcpyDeviceToHost, s));
-		CU_TRY(cudaStreamSynchronize(s));
-		for (size_t q = 0; q < nq; q++)
-		{
-			n_out[q] = (int32_t) hn[q];
-			for (size_t i = 0; i < k; i++)
-			{
-				const bool ok = i < hn[q];
-				if (!ok) labels_out[q * k + i] = ~(label_t) 0;
-				if (dists_out) dists_out[q * k + i] = ok ? o2f(hd[q * k + i]) : INFINITY;
-			}
-		}
-	}
-	if (tc)
-	{
-		g_scan_rescored += cnt[0];
-		g_scan_overflow += cnt[2];
-		if (cnt[1]) *tc_violation = true;
-	}
-	if (timing)
-		fprintf(stderr, "pgemb_scan_topk timing (ms): queries staged %.3f | kernels enqueued %.3f | kernels done %.3f | results copied + unpacked %.3f  (nq %zu, N %zu, %s)\n",
-				t_staged, t_enqueued, t_synced, since(), nq, N, tc ? "tensor-core filter" : "exact kernels");
-	return PGEMB_OK;
+	return scan_topk_groups(idx, nq, d_queries, k, d_labels_out, d_dists_out, d_n_out, true);
 }
 
 // Debug / test entry: the raw tensor-core products S[q][j] = q . row(r0 + j) of the K6 kernel (TF32 operands, fp32
@@ -1546,8 +1532,8 @@ extern "C" pgemb_status pgemb_debug_umma_product(pgemb_index *idx, size_t nq, co
 	if (st) return st;
 	stage.place(idx->d_stage);
 	cudaStream_t s = idx->stream;
-	CU_TRY(cudaMemsetAsync(d_q, 0, nq * rf * 4, s));
-	CU_TRY(cudaMemcpy2DAsync(d_q, rf * 4, queries, dim * 4, dim * 4, nq, cudaMemcpyHostToDevice, s));
+	st = stage_queries(idx, d_q, queries, nq, cudaMemcpyHostToDevice, s);
+	if (st) return st;
 	CU_TRY(cudaMemsetAsync(d_s, 0, nq * nr * 4, s));
 	st = ensure_row_norms(idx, s);
 	if (st) return st;

@@ -18,7 +18,7 @@
 //                             (dist_exact.cuh, one lane per candidate) and folded into the running top-k by (dist,label),
 //                             exactly like scan_select_kernel; then the query's filter constants are refreshed for the next chunk.
 //
-// The host (capi.cu, scan_topk_impl) walks the table in geometrically growing chunks (256, 512, 1K, ... rows): the first
+// The host (capi.cu, scan_filter_pass) walks the table in geometrically growing chunks (256, 512, 1K, ... rows): the first
 // chunk establishes the threshold, every later chunk is filtered with the exact threshold of everything before it, so
 // ~k ln(N/k) + (rows inside the error band) candidates per query are re-scored in total.  Result = the exact path's: same
 // labels, same order, bit-identical distances (tests/test_gpu_scan_umma.py).  Every re-scored candidate
