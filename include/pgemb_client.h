@@ -14,7 +14,8 @@
  *       records, read modified link lists back, mark labels deleted, truncate, drop.
  *
  * Concurrent hnsw_search calls of different backends are gathered by the sidecar into one batched traversal launch, and
- * concurrent index-less scans (pgemb_client_scan_topk) into one batched brute-force scan.
+ * concurrent index-less scans (pgemb_client_scan_topk) into one batched brute-force scan, and concurrent hnsw_dist_func
+ * calls into one batched distance launch.
  * All functions returning int return 0 on success and a pgemb_status (include/pgemb_b200.h) otherwise;
  * pgemb_client_last_error() describes the last failure of the calling thread.
  */
@@ -85,6 +86,11 @@ int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, 
 /* Sidecar scan counters, summed over replicas (largest batch: the maximum): pgemb_scan_topk calls, scans served, largest
  * batch.  Scans are not counted by pgemb_client_stats. */
 int pgemb_client_scan_stats(uint64_t *n_calls, uint64_t *n_scans, uint64_t *max_batch);
+/* Sidecar distance counters, summed over replicas (largest batch: the maximum): pgemb_dist_batch calls, hnsw_dist_func pairs
+ * served, largest batch.  The hnsw_dist_func calls that backends have pending at the same time for the same (metric, dim)
+ * are served by one pgemb_dist_batch call, each with the bits of a one-pair call.  Distances are not counted by
+ * pgemb_client_stats or pgemb_client_scan_stats. */
+int pgemb_client_dist_stats(uint64_t *n_calls, uint64_t *n_dists, uint64_t *max_batch);
 /* Ask the sidecar to exit (tests, controlled restarts). */
 int pgemb_client_shutdown_server(void);
 

@@ -517,6 +517,24 @@ int pgemb_client_scan_stats(uint64_t *n_calls, uint64_t *n_scans, uint64_t *max_
 	return PGEMB_OK;
 }
 
+int pgemb_client_dist_stats(uint64_t *n_calls, uint64_t *n_dists, uint64_t *max_batch)
+{
+	const int rc = ensure_connected();
+	if (rc) return rc;
+	uint64_t c = 0, d = 0, m = 0;
+	for (int i = 0; i < g_nconn; i++)
+	{
+		c += __atomic_load_n(&g_conn[i].hdr->n_dist_calls, __ATOMIC_RELAXED);
+		d += __atomic_load_n(&g_conn[i].hdr->n_dists, __ATOMIC_RELAXED);
+		const uint64_t mi = __atomic_load_n(&g_conn[i].hdr->max_dist_batch, __ATOMIC_RELAXED);
+		if (mi > m) m = mi;
+	}
+	if (n_calls) *n_calls = c;
+	if (n_dists) *n_dists = d;
+	if (max_batch) *max_batch = m;
+	return PGEMB_OK;
+}
+
 /* ---- the index-less scan (embedding.c:1022-1062 per row + the executor's sort; knn.out:63-91) ------------------------- */
 int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, label_t *labels_out, dist_t *dists_out, size_t *n_out)
 {

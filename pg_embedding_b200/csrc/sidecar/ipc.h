@@ -8,7 +8,7 @@
  * hnsw_search one query at a time (embedding.c:317,335); many backends doing so concurrently is exactly the batch the
  * traversal kernel wants, so the sidecar gathers the requests that are pending at the same time into ONE
  * pgemb_search_batch launch.  Index-less scans (PGEMB_OP_SCAN) are gathered the same way, per (relation, k), into one
- * pgemb_scan_topk call.
+ * pgemb_scan_topk call, and one-pair distances (PGEMB_OP_DIST), per (metric, dim), into one pgemb_dist_batch call.
  *
  * One POSIX shared-memory segment:
  *     IpcHeader | IpcSlot[n_slots] (each followed by its payload) | bulk area
@@ -28,7 +28,7 @@
 #include <stddef.h>
 
 #define PGEMB_IPC_MAGIC 0x424d4750u /* "PGMB" */
-#define PGEMB_IPC_VERSION 2u
+#define PGEMB_IPC_VERSION 3u
 
 enum
 {
@@ -79,6 +79,9 @@ typedef struct
 	uint64_t n_scan_calls;	 /* pgemb_scan_topk calls (scans are not counted in n_batches / n_searches / max_batch) */
 	uint64_t n_scans;		 /* scan queries served */
 	uint64_t max_scan_batch; /* largest scan batch so far */
+	uint64_t n_dist_calls;	 /* pgemb_dist_batch calls (distances are not counted in the search or scan counters) */
+	uint64_t n_dists;		 /* distance pairs served */
+	uint64_t max_dist_batch; /* largest distance batch so far */
 } PgembIpcHeader;
 
 typedef struct

@@ -6,8 +6,10 @@
 // (relation, efSearch) into ONE pgemb_search_batch launch: a single query cannot fill an H100, the concurrent queries
 // of many backends can (DESIGN.md section 6).  Index-less scans (`ORDER BY val <op> q LIMIT k` without the index) are
 // gathered the same way per (relation, k) into ONE pgemb_scan_topk call: every scan reads the whole table, so sharing
-// that read pays even more there (DESIGN.md section 12).  Everything else (mirror maintenance, hnsw_bind_point, link write-back)
-// is run one request at a time, which is also the reference's rule for writers (embedding.c:627-629: X-lock on page 0).
+// that read pays even more there (DESIGN.md section 12).  The SQL distance operators' hnsw_dist_func calls (one pair each,
+// embedding.c:1022-1062) are gathered per (metric, dim) into ONE pgemb_dist_batch call.  Everything else (mirror maintenance,
+// hnsw_bind_point, link write-back) is run one request at a time, which is also the reference's rule for writers
+// (embedding.c:627-629: X-lock on page 0).
 //
 // The library that does the work is dlopen()ed (--lib, default: libpgemb_b200.so next to this executable), so the
 // same binary serves the product library on the GPU and, in the CPU test-suite, the host-emulated build of it.
@@ -55,10 +57,10 @@ struct Api
 	pgemb_status (*reserve)(pgemb_index *, size_t);
 	pgemb_status (*search_batch)(pgemb_index *, size_t, const coord_t *, size_t, label_t *, dist_t *, idx_t *, int32_t *, uint32_t *);
 	pgemb_status (*scan_topk)(pgemb_index *, size_t, const coord_t *, size_t, label_t *, dist_t *, int32_t *);
+	pgemb_status (*dist_batch)(dist_func_t, size_t, size_t, const coord_t *, int, const coord_t *, dist_t *);
 	bool (*bind_point)(HnswMetadata *, const coord_t *, idx_t);	 // the reference-shaped hnsw_bind_point
 	pgemb_status (*build_bulk)(pgemb_index *, size_t, size_t, size_t, double *);
 	pgemb_status (*build_exact)(pgemb_index *, size_t, size_t, size_t, double *, uint64_t *);
-	dist_t (*dist_func)(dist_func_t, coord_t const *, coord_t const *, size_t);
 	void (*init_dist_func)(void);
 };
 
@@ -82,8 +84,8 @@ bool load_api(const char *path, Api &a)
 		   sym(h, "pgemb_index_capacity", a.index_capacity) && sym(h, "pgemb_index_append_records", a.append_records) &&
 		   sym(h, "pgemb_index_export_records", a.export_records) && sym(h, "pgemb_index_get_links", a.get_links) &&
 		   sym(h, "pgemb_index_set_labels", a.set_labels) && sym(h, "pgemb_index_truncate", a.truncate) && sym(h, "pgemb_index_reserve", a.reserve) && sym(h, "pgemb_search_batch", a.search_batch) &&
-		   sym(h, "pgemb_scan_topk", a.scan_topk) && sym(h, "hnsw_bind_point", a.bind_point) && sym(h, "pgemb_build_bulk", a.build_bulk) && sym(h, "pgemb_build_exact", a.build_exact) &&
-		   sym(h, "hnsw_dist_func", a.dist_func) && sym(h, "hnsw_init_dist_func", a.init_dist_func);
+		   sym(h, "pgemb_scan_topk", a.scan_topk) && sym(h, "pgemb_dist_batch", a.dist_batch) && sym(h, "hnsw_bind_point", a.bind_point) && sym(h, "pgemb_build_bulk", a.build_bulk) && sym(h, "pgemb_build_exact", a.build_exact) &&
+		   sym(h, "hnsw_init_dist_func", a.init_dist_func);
 }
 
 // ---- shared-memory helpers -----------------------------------------------------------------------------------------
@@ -123,6 +125,7 @@ struct Server
 	std::unordered_map<uint64_t, Mirror> mirrors;
 	// per-batch scratch
 	std::vector<float>	  qbuf;
+	std::vector<float>	  bbuf;	 // second vectors of the distance pairs
 	std::vector<label_t>  lbuf;
 	std::vector<float>	  dbuf;
 	std::vector<int32_t>  nbuf;
@@ -193,7 +196,7 @@ struct Server
 		return true;
 	}
 
-	// ---- everything except searches and scans: one at a time, in slot order ------------------------------------------
+	// ---- everything except searches, scans and distances: one at a time, in slot order ----------------------------
 	void run_control(PgembIpcSlot *s)
 	{
 		switch (s->op)
@@ -342,21 +345,6 @@ struct Server
 				finish_api(s, r);
 				return;
 			}
-			case PGEMB_OP_DIST:
-			{
-				const size_t dim = (size_t) s->a0;
-				if (dim < 1 || dim > hdr->max_dim || s->a1 > 2)
-				{
-					finish(s, PGEMB_ERR_ARG, "dist: bad dimension or metric");
-					return;
-				}
-				const float d = api.dist_func((dist_func_t) s->a1, slot_vec(s), slot_vec(s) + hdr->max_dim, dim);
-				uint32_t	bits;
-				memcpy(&bits, &d, 4);
-				s->a2 = bits;
-				finish(s, PGEMB_OK, nullptr);
-				return;
-			}
 			case PGEMB_OP_SHUTDOWN:
 				g_stop = 1;
 				finish(s, PGEMB_OK, nullptr);
@@ -457,12 +445,52 @@ struct Server
 		}
 	}
 
+	// ---- distances (hnsw_dist_func): all pending pairs of one (metric, dim) -> one pgemb_dist_batch per max_batch ----
+	// Every pair is independent and gets the bits of a one-pair call: the same dist_pairs_kernel evaluates each pair alone.
+	void run_dists(uint64_t metric, uint64_t dim, std::vector<PgembIpcSlot *> &group)
+	{
+		if (dim < 1 || dim > hdr->max_dim || metric > 2)
+		{
+			// the whole group shares the bad (metric, dim): each request fails by itself, the other groups are not affected
+			for (PgembIpcSlot *s : group) finish(s, PGEMB_ERR_ARG, "dist: bad dimension or metric");
+			return;
+		}
+		for (size_t lo = 0; lo < group.size(); lo += max_batch)
+		{
+			const size_t n = std::min(max_batch, group.size() - lo);
+			qbuf.resize(n * dim);
+			bbuf.resize(n * dim);
+			dbuf.resize(n);
+			for (size_t i = 0; i < n; i++)
+			{
+				memcpy(&qbuf[i * dim], slot_vec(group[lo + i]), dim * sizeof(float));
+				memcpy(&bbuf[i * dim], slot_vec(group[lo + i]) + hdr->max_dim, dim * sizeof(float));
+			}
+			const pgemb_status r = api.dist_batch((dist_func_t) metric, (size_t) dim, n, qbuf.data(), 0, bbuf.data(), dbuf.data());
+			hdr->n_dist_calls += 1;
+			hdr->n_dists += n;
+			if (n > hdr->max_dist_batch) hdr->max_dist_batch = n;
+			for (size_t i = 0; i < n; i++)
+			{
+				PgembIpcSlot *s = group[lo + i];
+				if (r == PGEMB_OK)
+				{
+					uint32_t bits;
+					memcpy(&bits, &dbuf[i], 4);
+					s->a2 = bits;
+				}
+				finish_api(s, r);
+			}
+		}
+	}
+
 	// one pass over the slots; returns the number of requests served
 	size_t serve_once()
 	{
 		std::vector<PgembIpcSlot *> control;
 		std::map<std::pair<uint64_t, uint32_t>, std::vector<PgembIpcSlot *>> searches;
 		std::map<std::pair<uint64_t, uint64_t>, std::vector<PgembIpcSlot *>> scans;
+		std::map<std::pair<uint64_t, uint64_t>, std::vector<PgembIpcSlot *>> dists;  // (metric, dim)
 		size_t found = 0, nsearch = 0;
 		auto   collect = [&]() {
 			  for (uint32_t i = 0; i < hdr->n_slots; i++)
@@ -478,12 +506,21 @@ struct Server
 				  }
 				  else if (s->op == PGEMB_OP_SCAN)
 					  scans[{s->index_key, s->a0}].push_back(s);  // not part of the searches' linger bookkeeping (nsearch / target / carry)
+				  else if (s->op == PGEMB_OP_DIST)
+					  dists[{s->a1, s->a0}].push_back(s);	 // touches no mirror, so no place in the write/search order; never lingers
 				  else
 					  control.push_back(s);
 			  }
 		};
+		// Distances first, as soon as they are collected: a one-pair request must not wait behind the searches' launches or
+		// their linger below.  Whatever queued up while the previous pass ran is served by one call per (metric, dim).
+		auto run_pending_dists = [&]() {
+			for (auto &kv : dists) run_dists(kv.first.first, kv.first.second, kv.second);
+			dists.clear();
+		};
 		collect();
 		if (found == 0) return 0;
+		run_pending_dists();
 		// Keeping the callers together.  A caller resubmits a few microseconds after it got its result, so a server that
 		// launches whatever is queued the moment it becomes free splits P steady callers into two groups that are served
 		// alternately -- each waits two launches per result.  `target` is the number of concurrent searchers the last
@@ -497,7 +534,11 @@ struct Server
 			if (0.25 * last_service_s > wait) wait = 0.25 * last_service_s;
 			if (wait > 2e-3) wait = 2e-3;
 			const double until = now_s() + wait;
-			while (nsearch < target && now_s() < until) collect();
+			while (nsearch < target && now_s() < until)
+			{
+				collect();
+				run_pending_dists();
+			}
 		}
 		for (PgembIpcSlot *s : control) run_control(s);
 		const double t_run = now_s();

@@ -2,9 +2,9 @@
 
 The sidecar is the one GPU-owning process of a forked-backend deployment (DESIGN.md section 12, INTEGRATION.md): it keeps
 the HBM mirror of every hnsw relation and gathers the one-query-per-call `hnsw_search` requests of concurrently running
-backends into batched traversal launches, and their index-less scans into batched brute-force scans.  This module is what
-tests/test_sidecar.py, tests/test_sidecar_scan.py and tools/bench_sidecar.py use; it contains no computation and no
-fallback -- without a serving sidecar every call fails.
+backends into batched traversal launches, their index-less scans into batched brute-force scans and their `hnsw_dist_func`
+calls into batched distance launches.  This module is what tests/test_sidecar*.py and tools/bench_sidecar.py use; it
+contains no computation and no fallback -- without a serving sidecar every call fails.
 """
 from __future__ import annotations
 
@@ -59,6 +59,7 @@ def client() -> C.CDLL:
     lib.pgemb_client_build.argtypes = [hp, sz, sz, sz, C.c_int, C.POINTER(C.c_double)]
     lib.pgemb_client_stats.argtypes = [C.POINTER(C.c_uint64)] * 3
     lib.pgemb_client_scan_stats.argtypes = [C.POINTER(C.c_uint64)] * 3
+    lib.pgemb_client_dist_stats.argtypes = [C.POINTER(C.c_uint64)] * 3
     lib.pgemb_client_scan_topk.argtypes = [hp, C.POINTER(C.c_float), sz, C.POINTER(C.c_uint64), C.POINTER(C.c_float), C.POINTER(sz)]
     lib.pgemb_client_set_interrupt_check.argtypes = [C.c_void_p]
     lib.hnsw_search.argtypes = [C.POINTER(HnswMetadata), C.POINTER(C.c_float), C.POINTER(sz), C.POINTER(C.POINTER(C.c_uint64))]
@@ -97,6 +98,14 @@ def scan_stats() -> dict:
     a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
     _check(client().pgemb_client_scan_stats(C.byref(a), C.byref(b), C.byref(c)))
     return {"calls": a.value, "scans": b.value, "max_batch": c.value}
+
+
+def dist_stats() -> dict:
+    """The sidecar's distance counters: pgemb_dist_batch calls, hnsw_dist_func pairs served, largest distance batch (not
+    part of stats() or scan_stats())."""
+    a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
+    _check(client().pgemb_client_dist_stats(C.byref(a), C.byref(b), C.byref(c)))
+    return {"calls": a.value, "dists": b.value, "max_batch": c.value}
 
 
 class RemoteIndex:

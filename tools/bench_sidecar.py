@@ -14,11 +14,32 @@ pgemb_client_scan_topk per call on the same table, no graph is built.  One JSON 
 percentiles, pgemb_scan_topk calls, mean and largest batch), then two lines timing pgemb_scan_topk in this process on the
 same table with nq = 1 and nq = 1024, for reference.  Every line names the GPU and its power limit.  Parity:
 tests/test_sidecar_scan.py.
+
+    python tools/bench_sidecar.py --op dist --dims 768 --metric cosine [--backends 1,16,64,256]
+
+measures the SQL distance operators evaluated per row (one hnsw_dist_func per call on random pairs, no table): one JSON line
+per backend count with distances/s, latency percentiles, pgemb_dist_batch calls, and mean and largest batch.
+
+    python tools/bench_sidecar.py --op search+dist --k 10 [--backends 1,16,64,256]
+
+models the projection query `SELECT id, val <=> q FROM t ORDER BY val <=> q LIMIT k` through the index: per call one
+hnsw_search at --efs, then --k hnsw_dist_func calls between the query and the returned rows' vectors.  Reports queries/s.
+
+    python tools/bench_sidecar.py --tree DIR ...
+
+runs the sidecar, the client library and their Python binding of another source tree (for example a checkout of an earlier
+commit, whose `pg_embedding_b200/build.py` builds its pgemb_sidecar and libpgemb_client.so), with this tree's
+libpgemb_b200.so.  Client and server always come from the same tree: the protocol version is checked at connect.  A tree
+without distance counters reports them as null; every line names the protocol version it ran.  Parity:
+tests/test_sidecar_dist.py.
 """
 import argparse
 import ctypes as C
 import json
+import math
 import os
+import shutil
+import struct
 import subprocess
 import sys
 import time
@@ -27,19 +48,26 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+METRICS = {"l2": 0, "cosine": 1, "manhattan": 2}
 
 
 def backend_main(a):
     """One backend: raw ctypes loop around hnsw_search (no numpy in the timed loop)."""
+    sys.path.insert(0, os.path.abspath(a.tree))
     from pg_embedding_b200 import sidecar
     sidecar.connect(a.shm)
+    lib = sidecar.client()
+    if a.op == "dist":
+        return dist_backend_loop(a, lib)
     idx = sidecar.RemoteIndex(1, a.dims, a.m, a.efc, a.efs, a.metric, capacity=1)
     rng = np.random.default_rng(1000 + a.backend_id)
     q = np.load(a.queries)
     q = np.ascontiguousarray(q[rng.permutation(q.shape[0])], dtype=np.float32)
-    lib = sidecar.client()
     if a.op == "scan":
         return scan_backend_loop(a, idx, lib, q)
+    rows = np.load(a.rows_file, mmap_mode="r") if a.op == "search+dist" else None   # the table, shared through the page cache
+    metric = METRICS[a.metric]
+    f32p = C.POINTER(C.c_float)
     free = C.CDLL(None).free
     free.argtypes = [C.c_void_p]
     n, res = C.c_size_t(), C.POINTER(C.c_uint64)()
@@ -55,8 +83,14 @@ def backend_main(a):
         t0 = time.perf_counter()
         if t0 >= t_end:
             break
-        if not lib.hnsw_search(meta, ptrs[i % len(ptrs)], C.byref(n), C.byref(res)):
+        qp = ptrs[i % len(ptrs)]
+        if not lib.hnsw_search(meta, qp, C.byref(n), C.byref(res)):
             raise RuntimeError(lib.pgemb_client_last_error().decode())
+        if rows is not None:
+            # the projection: the executor evaluates `val <op> q` once per returned row (embedding.c:1022-1062)
+            for j in range(min(a.k, n.value)):
+                if math.isnan(lib.hnsw_dist_func(metric, rows[res[j]].ctypes.data_as(f32p), qp, a.dims)):
+                    raise RuntimeError(lib.pgemb_client_last_error().decode())
         free(res)
         lat.append(time.perf_counter() - t0)
         i += 1
@@ -82,6 +116,31 @@ def scan_backend_loop(a, idx, lib, q):
         if t0 >= t_end:
             break
         if lib.pgemb_client_scan_topk(h, ptrs[i % len(ptrs)], a.k, labels, dists, C.byref(n)) != 0:
+            raise RuntimeError(lib.pgemb_client_last_error().decode())
+        lat.append(time.perf_counter() - t0)
+        i += 1
+    np.save(a.out, np.array(lat, np.float64))
+
+
+def dist_backend_loop(a, lib):
+    """One backend of --op dist: raw ctypes loop around hnsw_dist_func on random pairs (no numpy in the timed loop)."""
+    rng = np.random.default_rng(2000 + a.backend_id)
+    pairs = rng.standard_normal((256, 2, a.dims)).astype(np.float32) + (1.0 if a.metric == "cosine" else 0.0)
+    f32p = C.POINTER(C.c_float)
+    ptrs = [(p[0].ctypes.data_as(f32p), p[1].ctypes.data_as(f32p)) for p in pairs]
+    metric = METRICS[a.metric]
+    open(a.out + ".ready", "w").close()
+    while not os.path.exists(a.go):
+        time.sleep(0.001)
+    lat = []
+    t_end = time.perf_counter() + a.seconds
+    i = 0
+    while True:
+        t0 = time.perf_counter()
+        if t0 >= t_end:
+            break
+        pa, pb = ptrs[i % len(ptrs)]
+        if math.isnan(lib.hnsw_dist_func(metric, pa, pb, a.dims)):
             raise RuntimeError(lib.pgemb_client_last_error().decode())
         lat.append(time.perf_counter() - t0)
         i += 1
@@ -134,20 +193,39 @@ def main():
     ap.add_argument("--seconds", type=float, default=5.0)
     ap.add_argument("--linger-us", type=int, default=None, help="sidecar's --linger-us (default: the sidecar's own default)")
     ap.add_argument("--lib", default=None, help="C-ABI library the sidecar loads (default: the product library)")
-    ap.add_argument("--op", choices=("search", "scan"), default="search", help="search: hnsw_search per call; scan: pgemb_client_scan_topk per call")
-    ap.add_argument("--k", type=int, default=10, help="LIMIT of --op scan")
+    ap.add_argument("--op", choices=("search", "scan", "dist", "search+dist"), default="search",
+                    help="search: hnsw_search per call; scan: pgemb_client_scan_topk per call; dist: hnsw_dist_func per call; "
+                         "search+dist: hnsw_search then --k hnsw_dist_func per call")
+    ap.add_argument("--k", type=int, default=10, help="LIMIT of --op scan, distances per query of --op search+dist")
+    ap.add_argument("--tree", default=ROOT, help="source tree whose sidecar, client library and binding to run (default: this one)")
     ap.add_argument("--numpy-data", action="store_true", help="iid numpy data instead of bench.py's generator (no torch / CUDA in this process: emulated runs)")
     # internal: backend mode
     ap.add_argument("--backend-id", type=int, default=-1)
-    ap.add_argument("--shm"), ap.add_argument("--queries"), ap.add_argument("--out"), ap.add_argument("--go")
+    ap.add_argument("--shm"), ap.add_argument("--queries"), ap.add_argument("--out"), ap.add_argument("--go"), ap.add_argument("--rows-file")
     a = ap.parse_args()
     if a.backend_id >= 0:
         return backend_main(a)
 
-    from pg_embedding_b200 import build, sidecar
+    from pg_embedding_b200 import build
     build.build()
+    lib = a.lib
+    if os.path.abspath(a.tree) != ROOT:
+        # the other tree's sidecar and client over this tree's product library (whose kernels it then measures)
+        lib = lib or build.OUT
+        for m in [m for m in sys.modules if m == "pg_embedding_b200" or m.startswith("pg_embedding_b200.")]:
+            del sys.modules[m]
+        sys.path.insert(0, os.path.abspath(a.tree))
+        from pg_embedding_b200 import build as tree_build
+        tree_build.build_sidecar()
+    from pg_embedding_b200 import sidecar
+    assert os.path.dirname(os.path.abspath(sidecar.__file__)) == os.path.join(os.path.abspath(a.tree), "pg_embedding_b200")
+    dist_stats = getattr(sidecar, "dist_stats", None)      # None: a tree without distance counters
     X = None
-    if a.dims == 768 and not a.numpy_data:
+    if a.op == "dist":
+        rng = np.random.default_rng(1234)
+        X = np.zeros((0, a.dims), np.float32)               # no table: pairs are generated by the backends
+        Q = rng.standard_normal((1, a.dims)).astype(np.float32)
+    elif a.dims == 768 and not a.numpy_data:
         import bench  # the BASELINE data generator (clustered mixture, seeds 1234/5678)
         import torch
         X, Q = bench.make_data(torch, a.rows, 8192)
@@ -158,39 +236,43 @@ def main():
     X = X.cpu().numpy() if hasattr(X, "cpu") else X
     Q = Q.cpu().numpy() if hasattr(Q, "cpu") else Q
     shm = f"/pgemb_bench_{os.getpid()}"
-    srv = sidecar.SidecarProcess(shm, lib=a.lib, slots=512, bulk_mb=64, linger_us=a.linger_us)
+    srv = sidecar.SidecarProcess(shm, lib=lib, slots=512, bulk_mb=64, linger_us=a.linger_us)
     srv.wait_ready(120)
     tmp = f"/tmp/pgemb_bench_{os.getpid()}"
     os.makedirs(tmp, exist_ok=True)
     try:
-        idx = sidecar.RemoteIndex(1, a.dims, a.m, a.efc, a.efs, a.metric, capacity=a.rows)
+        protocol = struct.unpack_from("<I", open("/dev/shm" + shm, "rb").read(8), 4)[0]
+        idx = sidecar.RemoteIndex(1, a.dims, a.m, a.efc, a.efs, a.metric, capacity=max(X.shape[0], 1))
         rs = idx.record_bytes
         t0 = time.time()
         step = 16384  # 16384 x 3340 B = 55 MB per request: within the 64 MB bulk area
-        for lo in range(0, a.rows, step):
-            hi = min(a.rows, lo + step)
+        for lo in range(0, X.shape[0], step):
+            hi = min(X.shape[0], lo + step)
             rec = np.zeros((hi - lo, rs), np.uint8)
             rec[:, (2 * a.m + 1) * 4:(2 * a.m + 1) * 4 + a.dims * 4] = np.ascontiguousarray(X[lo:hi]).view(np.uint8)
             rec[:, rs - 8:] = np.arange(lo, hi, dtype=np.uint64).view(np.uint8).reshape(hi - lo, 8)
             idx.append_records(rec)
         t_ship = time.time() - t0
-        if a.op == "search":
+        if a.op in ("search", "search+dist"):
             t_build = idx.build(0, a.rows, batch_max=4096, exact=False)
             print(f"# shipped {a.rows} records in {t_ship:.1f}s, bulk build {t_build:.1f}s", file=sys.stderr)
-        else:
+        elif a.op == "scan":
             print(f"# shipped {a.rows} records in {t_ship:.1f}s (a scan needs no graph)", file=sys.stderr)
         info = gpu_info()
-        qf = os.path.join(tmp, "q.npy")
+        qf, xf = os.path.join(tmp, "q.npy"), os.path.join(tmp, "x.npy")
         np.save(qf, Q)
+        if a.op == "search+dist":
+            np.save(xf, np.ascontiguousarray(X, dtype=np.float32))
         for P in [int(x) for x in a.backends.split(",")]:
             go = os.path.join(tmp, f"go{P}")
-            s0 = sidecar.stats() if a.op == "search" else sidecar.scan_stats()
+            s0 = sidecar.scan_stats() if a.op == "scan" else sidecar.stats()
+            d0 = dist_stats() if dist_stats else None
             procs = []
             for b in range(P):
                 out = os.path.join(tmp, f"lat_{P}_{b}.npy")
                 cmd = [sys.executable, os.path.abspath(__file__), "--backend-id", str(b), "--shm", shm, "--queries", qf, "--out", out, "--go", go,
                        "--dims", str(a.dims), "--m", str(a.m), "--efc", str(a.efc), "--efs", str(a.efs), "--metric", a.metric, "--seconds", str(a.seconds),
-                       "--op", a.op, "--k", str(a.k)]
+                       "--op", a.op, "--k", str(a.k), "--tree", a.tree, "--rows-file", xf]
                 procs.append((subprocess.Popen(cmd), out))
             while not all(os.path.exists(o + ".ready") or p.poll() is not None for p, o in procs):
                 time.sleep(0.01)
@@ -207,8 +289,23 @@ def main():
                                   "workload": f"dims={a.dims} N={a.rows} {a.metric} LIMIT {a.k}, one pgemb_client_scan_topk per call per backend process",
                                   **info}), flush=True)
                 continue
+            d1 = dist_stats() if dist_stats else None
+            nd, ndc = (d1["dists"] - d0["dists"], d1["calls"] - d0["calls"]) if d1 else (None, None)
+            dist_batching = {"dist_batch_calls": ndc, "mean_dist_batch": round(nd / max(ndc, 1), 2) if d1 else None,
+                             "max_dist_batch_so_far": d1["max_batch"] if d1 else None, "protocol": protocol}
+            if a.op == "dist":
+                print(json.dumps({"op": "dist", "backends": P, "dists_per_s": round(lat.size / a.seconds, 1), "calls": int(lat.size),
+                                  "latency_ms": pct, **dist_batching,
+                                  "workload": f"dims={a.dims} {a.metric}, one hnsw_dist_func per call per backend process", **info}), flush=True)
+                continue
             s1 = sidecar.stats()
             nb, ns = s1["batches"] - s0["batches"], s1["searches"] - s0["searches"]
+            if a.op == "search+dist":
+                print(json.dumps({"op": "search+dist", "backends": P, "k": a.k, "queries_per_s": round(lat.size / a.seconds, 1), "calls": int(lat.size),
+                                  "latency_ms": pct, "launches": nb, "mean_batch": round(ns / max(nb, 1), 2), **dist_batching,
+                                  "workload": f"dims={a.dims} N={a.rows} {a.metric} m={a.m} efS={a.efs}, per call one hnsw_search and "
+                                              f"{a.k} hnsw_dist_func on the returned rows per backend process", **info}), flush=True)
+                continue
             print(json.dumps({"backends": P, "queries_per_s": round(lat.size / a.seconds, 1), "calls": int(lat.size),
                               "latency_ms": pct,
                               "launches": nb, "mean_batch": round(ns / max(nb, 1), 2), "max_batch_so_far": s1["max_batch"],
@@ -218,6 +315,7 @@ def main():
     finally:
         sidecar.client().pgemb_client_disconnect()
         srv.stop()
+        shutil.rmtree(tmp, ignore_errors=True)
 
 
 if __name__ == "__main__":
