@@ -127,8 +127,8 @@ struct pgemb_index
 	cudaStream_t stream = nullptr;
 	cudaEvent_t	 ev0 = nullptr, ev1 = nullptr;
 	static constexpr int kMaxChunks = 16;
-	cudaStream_t s_in = nullptr, s_out = nullptr;  // copy streams of the host-pointer batch API
-	cudaEvent_t	 ev_in[kMaxChunks] = {}, ev_k[kMaxChunks] = {};
+	cudaStream_t s_in = nullptr;  // copy stream of the host-pointer batch API
+	cudaEvent_t	 ev_in = nullptr;  // the traversal's stream waits on it for the queries (or the first `avail`) to land
 	unsigned int *h_avail = nullptr;  // pinned: values the copy stream publishes to the running kernel
 	bool		 ev_valid = false;
 	// search workspace
@@ -246,12 +246,7 @@ extern "C" void pgemb_index_destroy(pgemb_index *idx)
 	if (idx->stream) cudaStreamDestroy(idx->stream);
 	if (idx->s_in) cudaStreamDestroy(idx->s_in);
 	if (idx->h_avail) cudaFreeHost(idx->h_avail);
-	if (idx->s_out) cudaStreamDestroy(idx->s_out);
-	for (int i = 0; i < pgemb_index::kMaxChunks; i++)
-	{
-		if (idx->ev_in[i]) cudaEventDestroy(idx->ev_in[i]);
-		if (idx->ev_k[i]) cudaEventDestroy(idx->ev_k[i]);
-	}
+	if (idx->ev_in) cudaEventDestroy(idx->ev_in);
 	if (idx->ev0) cudaEventDestroy(idx->ev0);
 	if (idx->ev1) cudaEventDestroy(idx->ev1);
 	delete idx;
@@ -545,7 +540,7 @@ static int env_int(const char *name, int dflt)
 }
 
 // shared-memory layout + slots/rings per CTA: search_config.h (shared with the host emulation harness in tests/emu)
-static pgemb_status make_config(const pgemb_index *idx, uint32_t ef, SearchConfig *c, bool coop = false, bool res_global = false)
+static pgemb_status make_config(const pgemb_index *idx, uint32_t ef, SearchConfig *c, bool coop, bool res_global)
 {
 	SearchShape sh;
 	sh.res_global = res_global;
@@ -571,32 +566,6 @@ static pgemb_status make_config(const pgemb_index *idx, uint32_t ef, SearchConfi
 		case 1: return fail(PGEMB_ERR_CAPACITY, "search working set does not fit shared memory (dims/ef/maxM too large)");
 		default: return fail(PGEMB_ERR_CAPACITY, "PGEMB_WARPS/PGEMB_RINGS do not fit shared memory");
 	}
-}
-
-typedef void (*search_fn_t)(const SearchParams);
-
-static search_fn_t pick_search_kernel(int metric, bool coop, uint32_t tpr, bool res_global = false)
-{
-	if (res_global)
-	{
-		if (coop || tpr != 4) return nullptr;
-		switch (metric)
-		{
-			case DIST_L2: return search_kernel<M_L2, false, 4, true>;
-			case DIST_COSINE: return search_kernel<M_COS, false, 4, true>;
-			case DIST_MANHATTAN: return search_kernel<M_MAN, false, 4, true>;
-		}
-		return nullptr;
-	}
-	if (metric == DIST_L2 && tpr == 8) return coop ? search_kernel<M_L2, true, 8> : search_kernel<M_L2, false, 8>;
-	if (tpr != 4) return nullptr;
-	switch (metric)
-	{
-		case DIST_L2: return coop ? search_kernel<M_L2, true> : search_kernel<M_L2, false>;
-		case DIST_COSINE: return coop ? search_kernel<M_COS, true> : search_kernel<M_COS, false>;
-		case DIST_MANHATTAN: return coop ? search_kernel<M_MAN, true> : search_kernel<M_MAN, false>;
-	}
-	return nullptr;
 }
 
 // Visited-set sizing: an open-addressing table of vh entries per slot (kept at most half full by the
@@ -656,145 +625,105 @@ static pgemb_status ensure_workspace(pgemb_index *idx, uint32_t slots, uint32_t 
 	return PGEMB_OK;
 }
 
-// Launch the traversal for nq queries.  All pointers are device pointers.
-pgemb_status launch_search(pgemb_index *idx, size_t nq, const float *d_queries, uint32_t q_stride, const uint32_t *d_query_ids,
-						   uint32_t n_items, size_t ef, int raw_mode, label_t *d_labels_out, dist_t *d_dists_out, idx_t *d_ids_out,
-						   int32_t *d_n_out, uint32_t *d_stats_out, cudaStream_t s, bool time_it, const unsigned int *d_avail = nullptr, uint32_t *d_exp = nullptr,
-						   uint32_t exp_cap = 0, uint32_t *d_exp_n = nullptr)
+// Every decision of one traversal launch, made from the index, the batch size, ef and the PGEMB_* knobs (read on every call).
+struct SearchPlan
 {
-	if (!idx || !d_n_out) return fail(PGEMB_ERR_ARG, "null argument");
-	if (ef < 1 || ef > (1u << 27)) return fail(PGEMB_ERR_ARG, "ef out of range");
-	if (nq == 0) return PGEMB_OK;
-	if (nq >= (1ull << 31)) return fail(PGEMB_ERR_ARG, "too many queries in one batch");
-	pgemb_status st = set_device(idx);
-	if (st) return st;
-	// fewer queries than SMs: latency mode, a whole CTA cooperates on each query (search_kernel.cuh, COOP)
-	bool		 coop = nq <= (size_t) idx->sm_count && env_int("PGEMB_COOP", 1) != 0;
-	SearchConfig cfg;
-	bool		 res_global = env_int("PGEMB_RES_GLOBAL", 0) != 0;
-	if (res_global) coop = false;
-	st = make_config(idx, (uint32_t) ef, &cfg, coop, res_global);
-	if (st == PGEMB_ERR_CAPACITY && !res_global)
+	uint32_t	 ef = 0;
+	bool		 coop = false;		  // latency mode: a whole CTA cooperates on each query (search_kernel.cuh, COOP)
+	bool		 res_global = false;  // the result queues live in global memory (d_resg)
+	SearchConfig cfg;				  // slot-capped for res_global
+	search_fn_t	 fn = nullptr;
+	uint32_t	 vh = 0;  // visited-hash entries per slot (0: the bitmap alone)
+	uint32_t	 grid = 0;
+	bool		 pairs = false;	 // test both halves of a link list at once, if no list repeats an id
+	uint32_t	 prefetch_links = 1;
+	bool		 l2_window = false;	 // keep the per-slot hash sets resident in L2
+	bool		 fast_small = true;	 // skip the driver calls that would only restate what the last launch configured
+};
+
+static pgemb_status plan_search(const pgemb_index *idx, size_t nq, size_t ef, SearchPlan *pl)
+{
+	pl->ef = (uint32_t) ef;
+	pl->res_global = env_int("PGEMB_RES_GLOBAL", 0) != 0;
+	// fewer queries than SMs: latency mode
+	pl->coop = !pl->res_global && nq <= (size_t) idx->sm_count && env_int("PGEMB_COOP", 1) != 0;
+	pgemb_status st = make_config(idx, pl->ef, &pl->cfg, pl->coop, pl->res_global);
+	if (st == PGEMB_ERR_CAPACITY && !pl->res_global)
 	{
 		// 2 x ef result keys no longer fit a CTA's shared memory: the traversal variant that keeps them in global memory
 		// (throughput-mode kernel, 4 lanes per row) -- slower per hop, but efSearch doubling must not fail (embedding.c:334)
-		res_global = true;
-		coop = false;
-		st = make_config(idx, (uint32_t) ef, &cfg, false, true);
+		pl->res_global = true;
+		pl->coop = false;
+		st = make_config(idx, pl->ef, &pl->cfg, false, true);
 	}
 	if (st) return st;
-	if (res_global)
+	// small batches are spread over all SMs (the slots steal queries from one counter), not packed into few CTAs
+	pl->grid = (uint32_t) (nq < (size_t) idx->sm_count ? nq : (size_t) idx->sm_count);
+	pl->vh = visited_hash_entries(idx, pl->ef);
+	if (pl->res_global)
 	{
 		// per-slot global state is O(ef): cap the slots so that the workspace stays within ~4 GB
-		const uint64_t per_slot = (uint64_t) ef * 24u + (uint64_t) visited_hash_entries(idx, (uint32_t) ef) * 4u + ((uint64_t) idx->capacity + 31) / 32 * 4u;
-		uint64_t	   max_slots = ((uint64_t) 4 << 30) / (per_slot ? per_slot : 1);
-		if (max_slots < 1) max_slots = 1;
-		const uint64_t ctas = nq < (size_t) idx->sm_count ? nq : (size_t) idx->sm_count;
-		uint32_t	   w = (uint32_t) (max_slots / (ctas ? ctas : 1));
+		const uint64_t per_slot = (uint64_t) ef * 24u + (uint64_t) pl->vh * 4u + ((uint64_t) idx->capacity + 31) / 32 * 4u;
+		const uint64_t max_slots = ((uint64_t) 4 << 30) / (per_slot ? per_slot : 1);
+		uint32_t	   w = (uint32_t) (max_slots / (pl->grid ? pl->grid : 1));
 		if (w < 1) w = 1;
-		if (w < cfg.warps) cfg.warps = w;
-		cfg.slots = cfg.warps * (uint32_t) idx->sm_count;
+		if (w < pl->cfg.warps) pl->cfg.warps = w;
+		pl->cfg.slots = pl->cfg.warps * (uint32_t) idx->sm_count;
 	}
-	search_fn_t fn = pick_search_kernel((int) idx->meta.dist_func, coop, cfg.tpr, res_global);
-	if (!fn) return fail(PGEMB_ERR_ARG, "no kernel for this metric");
-	const bool fast_small = env_int("PGEMB_FAST_SMALL", 1) != 0;
-	if (!(fast_small && idx->last_fn == (const void *) fn && idx->last_smem == cfg.smem))
-	{
-		CU_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) cfg.smem));
-		int occ = 0;
-		CU_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, (int) cfg.warps * 32, cfg.smem));
-		if (occ < 1) return fail(PGEMB_ERR_CAPACITY, "search kernel cannot be resident (shared memory / registers)");
-		idx->last_fn = (const void *) fn;
-		idx->last_smem = cfg.smem;
-	}
-	const uint32_t slots = cfg.slots;
-	const uint32_t vh = visited_hash_entries(idx, (uint32_t) ef);
-	st = ensure_workspace(idx, slots, (uint32_t) ef, vh, cfg.vhs_entries);
-	if (st) return st;
-	if (res_global)
-	{
-		const size_t keys = (size_t) slots * 2 * ef;
-		if (idx->resg_keys < keys)
-		{
-			cudaFree(idx->d_resg);
-			idx->d_resg = nullptr;
-			idx->resg_keys = 0;
-			if (cudaMalloc((void **) &idx->d_resg, keys * 8) != cudaSuccess)
-			{
-				cudaGetLastError();
-				return fail(PGEMB_ERR_NOMEM, "out of device memory for the result queues of this efSearch");
-			}
-			idx->resg_keys = keys;
-		}
-	}
-
-	SearchParams p;
-	memset(&p, 0, sizeof(p));
-	p.vectors = idx->d_vectors;
-	p.links = idx->d_links;
-	p.labels = idx->d_labels;
-	p.norms = idx->d_norms;
-	p.n_items = n_items;
-	p.dim = (uint32_t) idx->meta.dim;
-	p.row_f = idx->row_f;
-	p.link_stride = idx->link_stride;
-	p.maxM = (uint32_t) idx->meta.maxM;
-	p.entry = idx->meta.enterpoint_node;
-	p.queries = d_queries;
-	p.query_ids = d_query_ids;
-	p.nq = (uint32_t) nq;
-	p.q_stride = q_stride;
-	p.ef = (uint32_t) ef;
-	p.raw_mode = raw_mode ? 1u : 0u;
-	p.labels_out = d_labels_out;
-	p.dists_out = d_dists_out;
-	p.ids_out = d_ids_out;
-	p.n_out = d_n_out;
-	p.stats_out = d_stats_out;
-	p.visited = idx->d_visited;
-	p.vlog = idx->d_vlog;
-	p.ovf = idx->d_ovf;
-	p.res_g = res_global ? idx->d_resg : nullptr;
-	p.vis_words = idx->vis_words;
-	p.vlog_cap = idx->vlog_cap;
-	p.vhash = idx->d_vhash;
-	p.vh_size = vh;
-	{
-		uint32_t lg = 0;
-		while ((1u << lg) < vh) lg++;
-		p.vh_shift = 32u - lg;
-	}
-	p.counter = idx->d_counter;
-	p.avail = d_avail;
-	p.exp_out = d_exp;
-	p.exp_cap = exp_cap;
-	p.exp_n_out = d_exp_n;
-	p.error_flag = idx->d_error;
-	apply_config(p, cfg, idx->row_f);
-	p.prefetch_links = (uint32_t) env_int("PGEMB_PREFETCH", 1);
+	pl->fn = pick_search_kernel((int) idx->meta.dist_func, pl->coop, pl->cfg.tpr, pl->res_global);
+	if (!pl->fn) return fail(PGEMB_ERR_ARG, "no kernel for this metric");
 	// latency mode: both 32-id halves of a link list are test-and-set concurrently (one round trip instead of two dependent
 	// ones) -- legal only when no list repeats an id, which holds for every list the bind kernels write and is checked once
 	// for lists that came from the caller.  (Throughput mode: measured slower, 0.82 vs 0.85 of the roofline -- not used there.)
-	p.visited_pairs = 0;
-	if (coop && env_int("PGEMB_VISITED_PAIRS", 1) != 0)
-	{
-		if (!idx->links_checked)
-		{
-			// caller-provided link lists: one pass to learn whether any list repeats an id (sticky until truncate)
-			const uint32_t nn = (uint32_t) idx->n;
-			int			   dup = 0;
-			CU_TRY(cudaMemsetAsync(idx->d_counter + 3, 0, sizeof(int), s));
-			if (nn) PGEMB_LAUNCH(links_distinct_kernel, (nn + 3) / 4, 128, 0, s, idx->d_links, idx->link_stride, (uint32_t) idx->meta.maxM, 0u, nn, (int *) (idx->d_counter + 3));
-			g_launches++;
-			CU_TRY(cudaMemcpyAsync(&dup, idx->d_counter + 3, sizeof(int), cudaMemcpyDeviceToHost, s));
-			CU_TRY(cudaStreamSynchronize(s));
-			idx->links_distinct = idx->links_distinct && dup == 0;
-			idx->links_checked = true;
-		}
-		p.visited_pairs = idx->links_distinct ? 1u : 0u;
-	}
+	pl->pairs = pl->coop && env_int("PGEMB_VISITED_PAIRS", 1) != 0;
+	pl->prefetch_links = (uint32_t) env_int("PGEMB_PREFETCH", 1);
+	pl->l2_window = pl->vh && idx->l2_window_max > 0 && env_int("PGEMB_L2_PERSIST", 1);
+	pl->fast_small = env_int("PGEMB_FAST_SMALL", 1) != 0;
+	return PGEMB_OK;
+}
 
-	if (vh && idx->l2_window_max > 0 && env_int("PGEMB_L2_PERSIST", 1))
+// The device state a launch of `pl` needs: the kernel's shared-memory attribute and residency, the workspace, the global result
+// queues, the link-list check and the L2 window.
+static pgemb_status prepare_search(pgemb_index *idx, const SearchPlan &pl, cudaStream_t s)
+{
+	if (!(pl.fast_small && idx->last_fn == (const void *) pl.fn && idx->last_smem == pl.cfg.smem))
+	{
+		CU_TRY(cudaFuncSetAttribute(pl.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) pl.cfg.smem));
+		int occ = 0;
+		CU_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pl.fn, (int) pl.cfg.warps * 32, pl.cfg.smem));
+		if (occ < 1) return fail(PGEMB_ERR_CAPACITY, "search kernel cannot be resident (shared memory / registers)");
+		idx->last_fn = (const void *) pl.fn;
+		idx->last_smem = pl.cfg.smem;
+	}
+	const pgemb_status st = ensure_workspace(idx, pl.cfg.slots, pl.ef, pl.vh, pl.cfg.vhs_entries);
+	if (st) return st;
+	const size_t keys = (size_t) pl.cfg.slots * 2 * pl.ef;
+	if (pl.res_global && idx->resg_keys < keys)
+	{
+		cudaFree(idx->d_resg);
+		idx->d_resg = nullptr;
+		idx->resg_keys = 0;
+		if (cudaMalloc((void **) &idx->d_resg, keys * 8) != cudaSuccess)
+		{
+			cudaGetLastError();
+			return fail(PGEMB_ERR_NOMEM, "out of device memory for the result queues of this efSearch");
+		}
+		idx->resg_keys = keys;
+	}
+	if (pl.pairs && !idx->links_checked)
+	{
+		// caller-provided link lists: one pass to learn whether any list repeats an id (sticky until truncate)
+		const uint32_t nn = (uint32_t) idx->n;
+		int			   dup = 0;
+		CU_TRY(cudaMemsetAsync(idx->d_counter + 3, 0, sizeof(int), s));
+		if (nn) PGEMB_LAUNCH(links_distinct_kernel, (nn + 3) / 4, 128, 0, s, idx->d_links, idx->link_stride, (uint32_t) idx->meta.maxM, 0u, nn, (int *) (idx->d_counter + 3));
+		g_launches++;
+		CU_TRY(cudaMemcpyAsync(&dup, idx->d_counter + 3, sizeof(int), cudaMemcpyDeviceToHost, s));
+		CU_TRY(cudaStreamSynchronize(s));
+		idx->links_distinct = idx->links_distinct && dup == 0;
+		idx->links_checked = true;
+	}
+	if (pl.l2_window)
 	{
 		if (idx->l2_limit_dropped)
 		{
@@ -802,36 +731,112 @@ pgemb_status launch_search(pgemb_index *idx, size_t nq, const float *d_queries, 
 			cudaGetLastError();
 			idx->l2_limit_dropped = false;
 		}
-		// keep the per-slot visited sets (hit on every hop by L2 atomics) resident while rows stream through L2
-		cudaStreamAttrValue av;
-		memset(&av, 0, sizeof(av));
-		size_t bytes = (size_t) slots * vh * 4;
+		// keep the per-slot visited sets (hit on every hop by L2 atomics) resident while rows stream through L2 -- unless the
+		// stream already carries exactly this window
+		size_t bytes = (size_t) pl.cfg.slots * pl.vh * 4;
 		if (bytes > idx->l2_window_max) bytes = idx->l2_window_max;
-		av.accessPolicyWindow.base_ptr = idx->d_vhash;
-		av.accessPolicyWindow.num_bytes = bytes;
-		av.accessPolicyWindow.hitRatio = 1.0f;
-		av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-		av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-		if (fast_small && idx->last_l2_base == (const void *) idx->d_vhash && idx->last_l2_bytes == bytes && idx->last_l2_stream == s)
+		if (!(pl.fast_small && idx->last_l2_base == (const void *) idx->d_vhash && idx->last_l2_bytes == bytes && idx->last_l2_stream == s))
 		{
-			// the stream already carries exactly this window
-		}
-		else
-		{
+			cudaStreamAttrValue av = {};
+			av.accessPolicyWindow.base_ptr = idx->d_vhash;
+			av.accessPolicyWindow.num_bytes = bytes;
+			av.accessPolicyWindow.hitRatio = 1.0f;
+			av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
+			av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
 			if (cudaStreamSetAttribute(s, cudaStreamAttributeAccessPolicyWindow, &av) != cudaSuccess) cudaGetLastError();
 			idx->last_l2_base = idx->d_vhash;
 			idx->last_l2_bytes = bytes;
 			idx->last_l2_stream = s;
 		}
 	}
+	return PGEMB_OK;
+}
+
+// What one traversal launch searches and where its results go (device pointers): caller vectors (`queries`, rows of dim floats;
+// timed for pgemb_last_kernel_ms) or stored nodes (`node_ids`: the build paths, raw mode, not timed).  `n` is required.
+struct SearchRequest
+{
+	SearchRequest(size_t nq, size_t ef, const float *queries, int32_t *n) : nq(nq), ef(ef), queries(queries), n(n) {}
+	SearchRequest(size_t nq, size_t ef, const uint32_t *node_ids, int32_t *n) : nq(nq), ef(ef), node_ids(node_ids), n(n) {}
+	size_t				nq, ef;
+	const float		   *queries = nullptr;
+	const uint32_t	   *node_ids = nullptr;
+	label_t			   *labels = nullptr;
+	dist_t			   *dists = nullptr;
+	idx_t			   *ids = nullptr;
+	int32_t			   *n = nullptr;
+	uint32_t		   *stats = nullptr;
+	const unsigned int *avail = nullptr;  // a batch streamed in next to the kernel (SearchParams::avail)
+	uint32_t		   *exp = nullptr, *exp_n = nullptr;  // pgemb_build_exact: each search's expansions (validate_kernel)
+	uint32_t			exp_cap = 0;
+};
+
+// One traversal launch: argument checks, plan_search, prepare_search, the parameter block, the launch.
+static pgemb_status launch_search(pgemb_index *idx, const SearchRequest &r, cudaStream_t s)
+{
+	if (!idx || !r.n) return fail(PGEMB_ERR_ARG, "null argument");
+	if (r.ef < 1 || r.ef > (1u << 27)) return fail(PGEMB_ERR_ARG, "ef out of range");
+	if (r.nq == 0) return PGEMB_OK;
+	if (r.nq >= (1ull << 31)) return fail(PGEMB_ERR_ARG, "too many queries in one batch");
+	pgemb_status st = set_device(idx);
+	if (st) return st;
+	SearchPlan pl;
+	st = plan_search(idx, r.nq, r.ef, &pl);
+	if (st) return st;
+	st = prepare_search(idx, pl, s);
+	if (st) return st;
+	const bool stored = r.node_ids != nullptr;
+	SearchParams p;
+	memset(&p, 0, sizeof(p));
+	p.vectors = idx->d_vectors;
+	p.links = idx->d_links;
+	p.labels = idx->d_labels;
+	p.norms = idx->d_norms;
+	p.n_items = (uint32_t) idx->n;
+	p.dim = (uint32_t) idx->meta.dim;
+	p.row_f = idx->row_f;
+	p.link_stride = idx->link_stride;
+	p.maxM = (uint32_t) idx->meta.maxM;
+	p.entry = idx->meta.enterpoint_node;
+	p.queries = r.queries;
+	p.query_ids = r.node_ids;
+	p.nq = (uint32_t) r.nq;
+	p.q_stride = stored ? 0u : p.dim;
+	p.ef = pl.ef;
+	p.raw_mode = stored ? 1u : 0u;
+	p.labels_out = r.labels;
+	p.dists_out = r.dists;
+	p.ids_out = r.ids;
+	p.n_out = r.n;
+	p.stats_out = r.stats;
+	p.visited = idx->d_visited;
+	p.vlog = idx->d_vlog;
+	p.ovf = idx->d_ovf;
+	p.res_g = pl.res_global ? idx->d_resg : nullptr;
+	p.vis_words = idx->vis_words;
+	p.vlog_cap = idx->vlog_cap;
+	p.vhash = idx->d_vhash;
+	p.vh_size = pl.vh;
+	{
+		uint32_t lg = 0;
+		while ((1u << lg) < pl.vh) lg++;
+		p.vh_shift = 32u - lg;
+	}
+	p.counter = idx->d_counter;
+	p.avail = r.avail;
+	p.exp_out = r.exp;
+	p.exp_cap = r.exp_cap;
+	p.exp_n_out = r.exp_n;
+	p.error_flag = idx->d_error;
+	apply_config(p, pl.cfg, idx->row_f);
+	p.prefetch_links = pl.prefetch_links;
+	p.visited_pairs = (pl.pairs && idx->links_distinct) ? 1u : 0u;
 	CU_TRY(cudaMemsetAsync(idx->d_counter, 0, sizeof(unsigned int), s));
-	// small batches are spread over all SMs (the slots steal queries from one counter), not packed into few CTAs
-	uint32_t grid = (uint32_t) (nq < (size_t) idx->sm_count ? nq : (size_t) idx->sm_count);
-	if (time_it) CU_TRY(cudaEventRecord(idx->ev0, s));
-	PGEMB_LAUNCH(fn, grid, cfg.warps * 32, cfg.smem, s, p);
+	if (!stored) CU_TRY(cudaEventRecord(idx->ev0, s));
+	PGEMB_LAUNCH(pl.fn, pl.grid, pl.cfg.warps * 32, pl.cfg.smem, s, p);
 	g_launches++;
 	CU_TRY(cudaGetLastError());
-	if (time_it)
+	if (!stored)
 	{
 		CU_TRY(cudaEventRecord(idx->ev1, s));
 		idx->ev_valid = true;
@@ -859,22 +864,100 @@ extern "C" pgemb_status pgemb_search_batch_device(pgemb_index *idx, size_t nq, c
 												  uint32_t *d_stats_out, void *stream)
 {
 	if (!idx) return fail(PGEMB_ERR_ARG, "null index");
-	return launch_search(idx, nq, d_queries, (uint32_t) idx->meta.dim, nullptr, (uint32_t) idx->n, ef, 0, d_labels_out, d_dists_out,
-						 d_ids_out, d_n_out, d_stats_out, (cudaStream_t) stream, true);
+	SearchRequest r(nq, ef, d_queries, d_n_out);
+	r.labels = d_labels_out;
+	r.dists = d_dists_out;
+	r.ids = d_ids_out;
+	r.stats = d_stats_out;
+	return launch_search(idx, r, (cudaStream_t) stream);
 }
 
-// Streaming the batch in behind the running kernel needs kernels and copies to overlap.  Tools that serialise
-// or replay kernel launches (Nsight Compute, compute-sanitizer: both arrive through CUDA_INJECTION64_PATH;
-// CUDA_LAUNCH_BLOCKING=1) get the plain copy-then-launch order.  PGEMB_STREAM_QUERIES=0/1 overrides.
-static bool stream_queries_enabled()
+struct HostOut { void *host; const void *dev; size_t bytes; };  // a caller's buffer (nullptr: not wanted), its part of the staging buffer
+
+// Enqueues the caller's queries to d_q on `s` (fast_small) or on the copy stream, streamed in chunks next to the kernel (*avail:
+// the count of queries landed so far) or whole before the launch.  *reader: the stream that reads the caller's buffer.
+static pgemb_status copy_queries_in(pgemb_index *idx, size_t nq, const coord_t *queries, float *d_q, bool fast_small, cudaStream_t s,
+									cudaStream_t *reader, const unsigned int **avail)
 {
-	const char *force = getenv("PGEMB_STREAM_QUERIES");
-	if (force && *force) return atoi(force) != 0;
-	const char *inj = getenv("CUDA_INJECTION64_PATH");
-	if (inj && *inj) return false;
-	const char *blk = getenv("CUDA_LAUNCH_BLOCKING");
-	if (blk && *blk && atoi(blk) != 0) return false;
-	return true;
+	const size_t dim = idx->meta.dim;
+	if (fast_small)
+	{
+		CU_TRY(cudaMemcpyAsync(d_q, queries, nq * dim * sizeof(float), cudaMemcpyHostToDevice, s));
+		return PGEMB_OK;
+	}
+	if (!idx->s_in)
+	{
+		CU_TRY(cudaStreamCreateWithFlags(&idx->s_in, cudaStreamNonBlocking));
+		CU_TRY(cudaEventCreateWithFlags(&idx->ev_in, cudaEventDisableTiming));
+		CU_TRY(cudaMallocHost((void **) &idx->h_avail, sizeof(unsigned int) * pgemb_index::kMaxChunks));
+	}
+	*reader = idx->s_in;
+	// Streaming the batch in behind the running kernel needs kernels and copies to overlap.  Tools that serialise or replay
+	// kernel launches (Nsight Compute, compute-sanitizer: both arrive through CUDA_INJECTION64_PATH; CUDA_LAUNCH_BLOCKING=1)
+	// get the plain copy-then-launch order.  PGEMB_STREAM_QUERIES=0/1 overrides.
+	const char	 *force = getenv("PGEMB_STREAM_QUERIES"), *inj = getenv("CUDA_INJECTION64_PATH");
+	const bool	  streamed = (force && *force) ? atoi(force) != 0 : !(inj && *inj) && env_int("CUDA_LAUNCH_BLOCKING", 0) == 0;
+	unsigned int *d_avail = idx->d_counter + 2;
+	size_t		  nchunks = streamed ? (nq + 4095) / 4096 : 1;
+	if (nchunks > (size_t) pgemb_index::kMaxChunks) nchunks = pgemb_index::kMaxChunks;
+	const size_t per = (nq + nchunks - 1) / nchunks;
+	CU_TRY(cudaMemsetAsync(d_avail, 0, sizeof(unsigned int), idx->s_in));
+	if (streamed)
+	{
+		// the kernel may start as soon as `avail` reads 0 ...
+		CU_TRY(cudaEventRecord(idx->ev_in, idx->s_in));
+		CU_TRY(cudaStreamWaitEvent(s, idx->ev_in, 0));
+		*avail = d_avail;
+	}
+	for (size_t c = 0, q0 = 0; q0 < nq; c++, q0 += per)
+	{
+		const size_t qn_ = (q0 + per <= nq) ? per : (nq - q0);
+		cudaError_t	 ce = cudaMemcpyAsync(d_q + q0 * dim, queries + q0 * dim, qn_ * dim * sizeof(float), cudaMemcpyHostToDevice, idx->s_in);
+		idx->h_avail[c] = (unsigned int) (q0 + qn_);
+		if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_avail, &idx->h_avail[c], sizeof(unsigned int), cudaMemcpyHostToDevice, idx->s_in);
+		if (ce != cudaSuccess) return fail(PGEMB_ERR_CUDA, std::string("pgemb_search_batch: copying the queries in failed: ") + cudaGetErrorString(ce));
+	}
+	if (!streamed)
+	{
+		// ... or, not streamed, only after the whole batch has landed
+		CU_TRY(cudaEventRecord(idx->ev_in, idx->s_in));
+		CU_TRY(cudaStreamWaitEvent(s, idx->ev_in, 0));
+	}
+	return PGEMB_OK;
+}
+
+// Ends a host-pointer search whose traversal is enqueued on `s`: the results go to the caller's buffers, the copy stream is
+// drained and the kernel's sticky error flag is read.  outs[0] .. outs[4] are back to back in the staging buffer.
+static pgemb_status search_hand_off(pgemb_index *idx, const HostOut (&outs)[5], bool fast_small, cudaStream_t s, cudaStream_t reader)
+{
+	// the outputs are one contiguous range of the staging buffer [labels | dists | ids | counts | stats]: after a small batch ONE
+	// copy into pinned memory + the 4-byte error flag, then one synchronisation (a copy into the caller's pageable buffers would
+	// block the host once per copy)
+	const char	*d_first = (const char *) outs[0].dev;
+	const size_t range = (size_t) ((const char *) outs[4].dev - d_first) + StageLayout::up(outs[4].bytes);
+	if (fast_small && range + 64 <= ((size_t) 4 << 20))
+	{
+		if (idx->land_bytes < range + 64)
+		{
+			if (idx->h_land) cudaFreeHost(idx->h_land);
+			idx->h_land = nullptr;
+			idx->land_bytes = 0;
+			CU_TRY(cudaMallocHost((void **) &idx->h_land, range + 64 + 65536));
+			idx->land_bytes = range + 64 + 65536;
+		}
+		int *h_err = (int *) (idx->h_land + ((range + 15) & ~(size_t) 15));
+		CU_TRY(cudaMemcpyAsync(idx->h_land, d_first, range, cudaMemcpyDeviceToHost, s));
+		CU_TRY(cudaMemcpyAsync(h_err, idx->d_error, sizeof(int), cudaMemcpyDeviceToHost, s));
+		CU_TRY(cudaStreamSynchronize(s));
+		for (const HostOut &o : outs)
+			if (o.host) memcpy(o.host, idx->h_land + ((const char *) o.dev - d_first), o.bytes);
+		if (*h_err != 0) return check_device_error(idx, s);	 // reads, reports and clears the flag
+		return PGEMB_OK;
+	}
+	for (const HostOut &o : outs)
+		if (o.host) CU_TRY(cudaMemcpyAsync(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost, s));
+	if (reader != s) CU_TRY(cudaStreamSynchronize(reader));
+	return check_device_error(idx, s);
 }
 
 extern "C" pgemb_status pgemb_search_batch(pgemb_index *idx, size_t nq, const coord_t *queries, size_t ef, label_t *labels_out,
@@ -884,25 +967,24 @@ extern "C" pgemb_status pgemb_search_batch(pgemb_index *idx, size_t nq, const co
 	if (nq == 0) return PGEMB_OK;
 	pgemb_status st = set_device(idx);
 	if (st) return st;
-	const size_t dim = idx->meta.dim;
 	const size_t lb = nq * ef * sizeof(uint64_t), db = nq * ef * sizeof(float), ib = nq * ef * sizeof(uint32_t);
 	const size_t nb = nq * sizeof(int32_t), sb = nq * 4 * sizeof(uint32_t);
 	float		*d_q = nullptr, *d_d = nullptr;
 	uint64_t	*d_l = nullptr;
 	uint32_t	*d_i = nullptr, *d_s = nullptr;
 	int32_t		*d_n = nullptr;
-	const StageLayout stage{{d_q, nq * dim * sizeof(float)}, {d_l, lb}, {d_d, db}, {d_i, ib}, {d_n, nb}, {d_s, sb}};
+	const StageLayout stage{{d_q, nq * idx->meta.dim * sizeof(float)}, {d_l, lb}, {d_d, db}, {d_i, ib}, {d_n, nb}, {d_s, sb}};
 	st = ensure_stage(idx, stage.bytes);
 	if (st) return st;
 	stage.place(idx->d_stage);
-	cudaStream_t s = idx->stream;
-	// the outputs the caller asked for, in staging order: [labels | dists | ids | counts | stats]
-	const struct { void *host; const void *dev; size_t bytes; } outs[5] = {{labels_out, d_l, lb}, {dists_out, d_d, db}, {ids_out, d_i, ib}, {n_out, d_n, nb}, {stats_out, d_s, sb}};
-	auto copy_out = [&]() -> pgemb_status {
-		for (const auto &o : outs)
-			if (o.host) CU_TRY(cudaMemcpyAsync(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost, s));
-		return PGEMB_OK;
-	};
+	cudaStream_t s = idx->stream, reader = s;
+	// the outputs the caller asked for, in staging order
+	const HostOut outs[5] = {{labels_out, d_l, lb}, {dists_out, d_d, db}, {ids_out, d_i, ib}, {n_out, d_n, nb}, {stats_out, d_s, sb}};
+	SearchRequest r(nq, ef, d_q, d_n);
+	r.labels = labels_out ? d_l : nullptr;
+	r.dists = dists_out ? d_d : nullptr;
+	r.ids = ids_out ? d_i : nullptr;
+	r.stats = stats_out ? d_s : nullptr;
 	// ONE traversal launch; the query batch is streamed in next to it: the copy stream moves chunk after chunk
 	// H2D and publishes "queries available" after each, the kernel's slots wait for their query to land
 	// (SearchParams::avail).  So the PCIe transfer hides behind the traversal instead of preceding it.
@@ -910,95 +992,14 @@ extern "C" pgemb_status pgemb_search_batch(pgemb_index *idx, size_t nq, const co
 	// blocking launch (CUDA_LAUNCH_BLOCKING, a profiler or sanitizer serialising kernels) cannot leave the kernel
 	// waiting for data that was never queued.  Under such a tool (detected by its injection variable) the batch is
 	// simply copied before the launch: replayed kernels must not depend on a concurrent copy.
-	if (env_int("PGEMB_FAST_SMALL", 1) != 0 && nq <= 64)
-	{
-		// a handful of queries (the reference-shaped hnsw_search: one) are not worth the streaming protocol
-		// -- copy, launch, copy back on ONE stream, one synchronisation
-		CU_TRY(cudaMemcpyAsync(d_q, queries, nq * dim * sizeof(float), cudaMemcpyHostToDevice, s));
-		st = launch_search(idx, nq, d_q, (uint32_t) dim, nullptr, (uint32_t) idx->n, ef, 0, labels_out ? d_l : nullptr, dists_out ? d_d : nullptr,
-						   ids_out ? d_i : nullptr, d_n, stats_out ? d_s : nullptr, s, true, nullptr);
-		if (st)
-		{
-			cudaStreamSynchronize(s);  // the caller's query buffer must not be read after we return
-			return st;
-		}
-		// the outputs are one contiguous range of the staging buffer [labels | dists | ids | counts | stats]: ONE copy into pinned
-		// memory + the 4-byte error flag, then one synchronisation (a copy into the caller's pageable buffers would block the host
-		// once per copy)
-		const size_t range = (size_t) ((char *) d_s - (char *) d_l) + StageLayout::up(sb);
-		if (range + 64 <= ((size_t) 4 << 20))
-		{
-			if (idx->land_bytes < range + 64)
-			{
-				if (idx->h_land) cudaFreeHost(idx->h_land);
-				idx->h_land = nullptr;
-				idx->land_bytes = 0;
-				CU_TRY(cudaMallocHost((void **) &idx->h_land, range + 64 + 65536));
-				idx->land_bytes = range + 64 + 65536;
-			}
-			int *h_err = (int *) (idx->h_land + ((range + 15) & ~(size_t) 15));
-			CU_TRY(cudaMemcpyAsync(idx->h_land, d_l, range, cudaMemcpyDeviceToHost, s));
-			CU_TRY(cudaMemcpyAsync(h_err, idx->d_error, sizeof(int), cudaMemcpyDeviceToHost, s));
-			CU_TRY(cudaStreamSynchronize(s));
-			for (const auto &o : outs)
-				if (o.host) memcpy(o.host, idx->h_land + ((const char *) o.dev - (const char *) d_l), o.bytes);
-			if (*h_err != 0) return check_device_error(idx, s);	 // reads, reports and clears the flag
-			return PGEMB_OK;
-		}
-		st = copy_out();
-		if (st) return st;
-		return check_device_error(idx, s);
-	}
-	if (!idx->s_in)
-	{
-		CU_TRY(cudaStreamCreateWithFlags(&idx->s_in, cudaStreamNonBlocking));
-		CU_TRY(cudaEventCreateWithFlags(&idx->ev_in[0], cudaEventDisableTiming));
-		CU_TRY(cudaMallocHost((void **) &idx->h_avail, sizeof(unsigned int) * pgemb_index::kMaxChunks));
-	}
-	const bool	  streamed = stream_queries_enabled();
-	unsigned int *d_avail = idx->d_counter + 2;
-	size_t		  nchunks = streamed ? (nq + 4095) / 4096 : 1;
-	if (nchunks > (size_t) pgemb_index::kMaxChunks) nchunks = pgemb_index::kMaxChunks;
-	const size_t per = (nq + nchunks - 1) / nchunks;
-	CU_TRY(cudaMemsetAsync(d_avail, 0, sizeof(unsigned int), idx->s_in));
-	if (streamed)
-	{
-		// the kernel may start as soon as `avail` reads 0 ...
-		CU_TRY(cudaEventRecord(idx->ev_in[0], idx->s_in));
-		CU_TRY(cudaStreamWaitEvent(s, idx->ev_in[0], 0));
-	}
-	cudaError_t ce = cudaSuccess;
-	for (size_t c = 0; c < nchunks && ce == cudaSuccess; c++)
-	{
-		const size_t q0 = c * per;
-		if (q0 >= nq) break;
-		const size_t qn_ = (q0 + per <= nq) ? per : (nq - q0);
-		ce = cudaMemcpyAsync(d_q + q0 * dim, queries + q0 * dim, qn_ * dim * sizeof(float), cudaMemcpyHostToDevice, idx->s_in);
-		idx->h_avail[c] = (unsigned int) (q0 + qn_);
-		if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_avail, &idx->h_avail[c], sizeof(unsigned int), cudaMemcpyHostToDevice, idx->s_in);
-	}
-	if (ce != cudaSuccess)
-	{
-		cudaStreamSynchronize(idx->s_in);  // nothing was launched; the caller's buffer must not be read after we return
-		return fail(PGEMB_ERR_CUDA, std::string("pgemb_search_batch: copying the queries in failed: ") + cudaGetErrorString(ce));
-	}
-	if (!streamed)
-	{
-		// ... or, not streamed, only after the whole batch has landed
-		CU_TRY(cudaEventRecord(idx->ev_in[0], idx->s_in));
-		CU_TRY(cudaStreamWaitEvent(s, idx->ev_in[0], 0));
-	}
-	st = launch_search(idx, nq, d_q, (uint32_t) dim, nullptr, (uint32_t) idx->n, ef, 0, labels_out ? d_l : nullptr, dists_out ? d_d : nullptr,
-					   ids_out ? d_i : nullptr, d_n, stats_out ? d_s : nullptr, s, true, streamed ? d_avail : nullptr);
-	if (st)
-	{
-		cudaStreamSynchronize(idx->s_in);
-		return st;
-	}
-	st = copy_out();
-	if (st) return st;
-	CU_TRY(cudaStreamSynchronize(idx->s_in));
-	return check_device_error(idx, s);
+	// A handful of queries (the reference-shaped hnsw_search: one) are not worth the streaming protocol: copy, launch, copy back
+	// on ONE stream, one synchronisation.
+	const bool fast_small = env_int("PGEMB_FAST_SMALL", 1) != 0 && nq <= 64;
+	st = copy_queries_in(idx, nq, queries, d_q, fast_small, s, &reader, &r.avail);
+	if (!st) st = launch_search(idx, r, s);
+	if (!st) st = search_hand_off(idx, outs, fast_small, s, reader);
+	if (st) cudaStreamSynchronize(reader);	// the caller's query buffer must not be read after we return
+	return st;
 }
 
 // The device-pointer entry points are asynchronous and do not read the kernel's sticky error flag; a caller that wants to know
@@ -1319,7 +1320,7 @@ static pgemb_status stage_queries(const pgemb_index *idx, float *d_q, const coor
 static pgemb_status scan_filter_pass(pgemb_index *idx, const ScanPlan &p, const ScanBuffers &b, size_t nq, size_t k, cudaStream_t s)
 {
 	// The filter lives on L2 reuse (the table streams from HBM once, the other query tiles re-read it from L2).  A traversal
-	// on this index leaves an L2 persistence window behind (the per-slot visited sets, launch_search): give those lines and
+	// on this index leaves an L2 persistence window behind (the per-slot visited sets, prepare_search): give those lines and
 	// the set-aside back before scanning.
 	if (p.l2reset > 0 && idx->last_l2_base != nullptr)
 	{
@@ -1867,6 +1868,23 @@ static pgemb_status launch_connect(pgemb_index *idx, const uint32_t *d_new_ids, 
 	return launch_backlinks(idx, count, s);
 }
 
+// Search `count` stored nodes (their ids at d_ids) with ef = efc into bind_ws slots [0,count); with_expansions: also record each
+// search's expansions for validate_kernel.
+static pgemb_status search_stored(pgemb_index *idx, const uint32_t *d_ids, size_t count, size_t efc, cudaStream_t s, bool with_expansions)
+{
+	BindWorkspace &w = idx->bind_ws;
+	SearchRequest  r(count, efc, d_ids, w.d_cand_n);
+	r.dists = w.d_cand_d;
+	r.ids = w.d_cand_ids;
+	if (with_expansions)
+	{
+		r.exp = w.d_exp;
+		r.exp_n = w.d_exp_n;
+		r.exp_cap = BindWorkspace::kExpCap;
+	}
+	return launch_search(idx, r, s);
+}
+
 __global__ void iota_kernel(uint32_t *out, uint32_t start, uint32_t n);
 
 pgemb_status bind_points(pgemb_index *idx, idx_t first, size_t n)
@@ -1879,7 +1897,6 @@ pgemb_status bind_points(pgemb_index *idx, idx_t first, size_t n)
 	// one bind at a time uses ONE slot of the bind workspace (candidates, pairs); only the ids are per point
 	pgemb_status st = ensure_bind_ws(idx, 1, efc);
 	if (st) return st;
-	BindWorkspace &w = idx->bind_ws;
 	if (idx->seq_ids_cap < n)
 	{
 		cudaFree(idx->d_seq_ids);
@@ -1895,8 +1912,7 @@ pgemb_status bind_points(pgemb_index *idx, idx_t first, size_t n)
 	for (size_t i = 0; i < n; i++)
 	{
 		if (first + i == 0) continue;  // hnswalg.cpp:227-228
-		st = launch_search(idx, 1, nullptr, 0, idx->d_seq_ids + i, (uint32_t) idx->n, efc, 1, nullptr, w.d_cand_d, w.d_cand_ids, w.d_cand_n,
-						   nullptr, s, false);
+		st = search_stored(idx, idx->d_seq_ids + i, 1, efc, s, false);
 		if (st) return st;
 		st = launch_connect(idx, idx->d_seq_ids + i, 1, efc, s);
 		if (st) return st;
@@ -1968,8 +1984,7 @@ extern "C" pgemb_status pgemb_build_bulk(pgemb_index *idx, size_t first, size_t 
 		}
 		PGEMB_LAUNCH(iota_kernel, (uint32_t) ((B + 255) / 256), 256, 0, s, w.d_qids, (uint32_t) pos, (uint32_t) B);
 		g_launches++;
-		st = launch_search(idx, B, nullptr, 0, w.d_qids, (uint32_t) idx->n, efc, 1, nullptr, w.d_cand_d, w.d_cand_ids, w.d_cand_n, nullptr, s,
-						   false);
+		st = search_stored(idx, w.d_qids, B, efc, s, false);
 		if (st) return st;
 		st = launch_connect(idx, w.d_qids, B, efc, s);
 		if (st) return st;
@@ -2032,8 +2047,7 @@ extern "C" pgemb_status pgemb_build_exact(pgemb_index *idx, size_t first, size_t
 		if (B > end - pos) B = end - pos;
 		PGEMB_LAUNCH(iota_kernel, (uint32_t) ((B + 255) / 256), 256, 0, s, w.d_qids, (uint32_t) pos, (uint32_t) B);
 		g_launches++;
-		st = launch_search(idx, B, nullptr, 0, w.d_qids, (uint32_t) idx->n, efc, 1, nullptr, w.d_cand_d, w.d_cand_ids, w.d_cand_n, nullptr, s,
-						   false, nullptr, w.d_exp, ecap, w.d_exp_n);
+		st = search_stored(idx, w.d_qids, B, efc, s, true);
 		if (st) return st;
 		batches++;
 		searches += B;
@@ -2330,8 +2344,10 @@ extern "C" pgemb_status pgemb_sharded_search_device(pgemb_index *idx, pgemb_exch
 	pgemb_status st = check_local_step(idx, ex, nq, ef, "ef");
 	if (st) return st;
 	const PackedTopk out = packed_topk(step_area(ex, ex->d_buf, ex->seq + 1), nq, ex->k);
-	st = launch_search(idx, nq, d_queries, (uint32_t) idx->meta.dim, nullptr, (uint32_t) idx->n, ef, 0, out.labels, out.dists, nullptr, out.counts, nullptr,
-					   (cudaStream_t) stream, true);
+	SearchRequest r(nq, ef, d_queries, out.counts);
+	r.labels = out.labels;
+	r.dists = out.dists;
+	st = launch_search(idx, r, (cudaStream_t) stream);
 	if (st) return st;
 	return publish_step(ex, (cudaStream_t) stream);
 }

@@ -357,7 +357,7 @@ __device__ __forceinline__ void coop_gather(const SearchParams &p, unsigned char
 }
 
 // RESG: the two result buffers of a slot live in global memory (p.res_g) instead of its shared-memory block -- the variant
-// launch_search falls back to when 2 x ef keys no longer fit a CTA, so that the caller's efSearch doubling (embedding.c:334)
+// plan_search (capi.cu) falls back to when 2 x ef keys no longer fit a CTA, so that the caller's efSearch doubling (embedding.c:334)
 // never fails before ef reaches the index size.  Same code path otherwise (the queue update then runs at L2 latency).
 template <int METRIC, bool COOP, int TPR = 4, bool RESG = false>
 __global__ void __launch_bounds__(1024) search_kernel(const SearchParams p)
@@ -1087,6 +1087,34 @@ __global__ void __launch_bounds__(1024) search_kernel(const SearchParams p)
 	}
 	// an unconsumed link prefetch must land before the CTA (and its shared memory) goes away
 	if (pf_inflight) mbar_wait(pf_bar, pf_parity);
+}
+
+typedef void (*search_fn_t)(const SearchParams);
+
+// The traversal instance for a metric, mode, lanes per row and result-queue placement (nullptr: there is none).  Host code,
+// shared by capi.cu's plan_search and the emulation harness in tests/emu, so that both launch the same instance.
+inline search_fn_t pick_search_kernel(int metric, bool coop, uint32_t tpr, bool res_global)
+{
+	if (res_global)
+	{
+		if (coop || tpr != 4) return nullptr;
+		switch (metric)
+		{
+			case DIST_L2: return search_kernel<M_L2, false, 4, true>;
+			case DIST_COSINE: return search_kernel<M_COS, false, 4, true>;
+			case DIST_MANHATTAN: return search_kernel<M_MAN, false, 4, true>;
+		}
+		return nullptr;
+	}
+	if (metric == DIST_L2 && tpr == 8) return coop ? search_kernel<M_L2, true, 8> : search_kernel<M_L2, false, 8>;
+	if (tpr != 4) return nullptr;
+	switch (metric)
+	{
+		case DIST_L2: return coop ? search_kernel<M_L2, true> : search_kernel<M_L2, false>;
+		case DIST_COSINE: return coop ? search_kernel<M_COS, true> : search_kernel<M_COS, false>;
+		case DIST_MANHATTAN: return coop ? search_kernel<M_MAN, true> : search_kernel<M_MAN, false>;
+	}
+	return nullptr;
 }
 
 }  // namespace pgemb

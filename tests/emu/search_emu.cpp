@@ -1,5 +1,6 @@
 // pgemb::search_kernel (throughput and latency mode) on the host SIMT emulator (tests/emu).
-// The harness plays the part of capi.cu's launch_search: same make_search_config, same parameter block.
+// The harness plays the part of capi.cu's plan_search and launch_search: same make_search_config, same pick_search_kernel,
+// same parameter block.
 #include <cuda_runtime.h>  // the stand-in in tests/emu/fake_cuda
 
 #include "../../pg_embedding_b200/csrc/bind_kernel.cuh"
@@ -12,11 +13,6 @@ extern "C" int emu_search_ex(int metric, int coop, const float *vectors, const u
 							 uint32_t nq, uint32_t ef, int raw_mode, uint64_t *labels_out, float *dists_out, uint32_t *ids_out,
 							 int32_t *n_out, uint32_t *stats_out, uint32_t want_warps, uint32_t want_rings, uint32_t grid, uint32_t vh_size,
 							 uint32_t visited_pairs, uint32_t smem_visited, int *error_out);
-
-template <int METRIC, bool COOP, int TPR = 4, bool RESG = false> static void go(const SearchParams &p, unsigned grid, unsigned warps, size_t smem)
-{
-	emu::launch(dim3(grid), warps * 32, smem, [=]() { search_kernel<METRIC, COOP, TPR, RESG>(p); });
-}
 
 // returns 0 on success, >0 = make_search_config's code, -1 = bad metric; *error_out = the kernel's sticky error flag
 extern "C" int emu_search(int metric, int coop, const float *vectors, const uint32_t *links, const uint64_t *labels, const float *norms,
@@ -108,28 +104,10 @@ extern "C" int emu_search_ex(int metric, int coop, const float *vectors, const u
 	apply_config(p, cfg, row_f);
 	unsigned g = nq < grid ? nq : grid;
 	if (g == 0) g = 1;
-	if (res_global)
-	{
-		if (coop || cfg.tpr != 4) return 79;
-		if (metric == 0) go<M_L2, false, 4, true>(p, g, cfg.warps, cfg.smem);
-		else if (metric == 1) go<M_COS, false, 4, true>(p, g, cfg.warps, cfg.smem);
-		else go<M_MAN, false, 4, true>(p, g, cfg.warps, cfg.smem);
-	}
-	else if (cfg.tpr == 8)
-	{
-		if (coop) go<M_L2, true, 8>(p, g, cfg.warps, cfg.smem); else go<M_L2, false, 8>(p, g, cfg.warps, cfg.smem);
-	}
-	else
-	switch (metric * 2 + (coop ? 1 : 0))
-	{
-		case 0: go<M_L2, false>(p, g, cfg.warps, cfg.smem); break;
-		case 1: go<M_L2, true>(p, g, cfg.warps, cfg.smem); break;
-		case 2: go<M_COS, false>(p, g, cfg.warps, cfg.smem); break;
-		case 3: go<M_COS, true>(p, g, cfg.warps, cfg.smem); break;
-		case 4: go<M_MAN, false>(p, g, cfg.warps, cfg.smem); break;
-		case 5: go<M_MAN, true>(p, g, cfg.warps, cfg.smem); break;
-		default: return -1;
-	}
+	if (res_global && (coop || cfg.tpr != 4)) return 79;
+	const search_fn_t fn = pick_search_kernel(metric, coop != 0, cfg.tpr, res_global);
+	if (!fn) return -1;
+	PGEMB_LAUNCH(fn, g, cfg.warps * 32, cfg.smem, 0, p);
 	// the visited sets must be left clean for the next launch
 	for (uint32_t v : visited)
 		if (v != 0u) err |= 0x100;
@@ -226,16 +204,9 @@ extern "C" int emu_bind_sequence(int metric, int coop, const float *vectors, uin
 		p.error_flag = &err;
 		p.prefetch_links = 1;
 		apply_config(p, cfg, row_f);
-		switch (metric * 2 + (coop ? 1 : 0))
-		{
-			case 0: go<M_L2, false>(p, 1, cfg.warps, cfg.smem); break;
-			case 1: go<M_L2, true>(p, 1, cfg.warps, cfg.smem); break;
-			case 2: go<M_COS, false>(p, 1, cfg.warps, cfg.smem); break;
-			case 3: go<M_COS, true>(p, 1, cfg.warps, cfg.smem); break;
-			case 4: go<M_MAN, false>(p, 1, cfg.warps, cfg.smem); break;
-			case 5: go<M_MAN, true>(p, 1, cfg.warps, cfg.smem); break;
-			default: return -1;
-		}
+		const search_fn_t fn = pick_search_kernel(metric, coop != 0, cfg.tpr, false);
+		if (!fn) return -1;
+		PGEMB_LAUNCH(fn, 1, cfg.warps * 32, cfg.smem, 0, p);
 		if (metric == 0) connect_one<M_L2>(g, &id, cand_ids.data(), cand_d.data(), &cand_n, efc, pairs.data());
 		else if (metric == 1) connect_one<M_COS>(g, &id, cand_ids.data(), cand_d.data(), &cand_n, efc, pairs.data());
 		else connect_one<M_MAN>(g, &id, cand_ids.data(), cand_d.data(), &cand_n, efc, pairs.data());

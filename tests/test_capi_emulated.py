@@ -526,7 +526,7 @@ def test_device_scan_edge_cases(pg, oracle_mod):
 
 
 def test_ef_beyond_shared_memory(pg, G, oracle_mod, monkeypatch):
-    """ef = 20000 through the library on the host: launch_search must fall back to the global-memory result queues by itself;
+    """ef = 20000 through the library on the host: plan_search must fall back to the global-memory result queues by itself;
     PGEMB_RES_GLOBAL=1 forces that variant for ordinary searches too."""
     G.check_ef_beyond_shared_memory(pg, oracle_mod, 12, 300, (20000, 64))
     monkeypatch.setenv("PGEMB_RES_GLOBAL", "1")

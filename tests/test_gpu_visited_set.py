@@ -69,7 +69,7 @@ def vlog_cap(capacity, vh_max, vhs=0):
 
 
 def set_knobs(monkeypatch, **kv):
-    """Every visited-set switch of launch_search set for this call: the given PGEMB_<name> values, the rest at their defaults."""
+    """Every visited-set switch of plan_search set for this call: the given PGEMB_<name> values, the rest at their defaults."""
     for k in KNOBS:
         v = kv.get(k)
         if v is None:

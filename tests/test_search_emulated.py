@@ -149,7 +149,7 @@ def test_search_kernel_emulated_very_large_ef(emu, oracle_mod, coop):
 
 @pytest.mark.parametrize("case", CASES, ids=[f"{c[0]}-d{c[1]}m{c[2]}" for c in CASES])
 def test_result_queues_in_global_memory(emu, oracle_mod, case):
-    """search_kernel<..., RESG>: the variant launch_search falls back to when 2 x ef keys do not fit shared memory (no ef ceiling:
+    """search_kernel<..., RESG>: the variant plan_search falls back to when 2 x ef keys do not fit shared memory (no ef ceiling:
     the reference doubles efSearch without bound, embedding.c:334).  Same labels, distances and traversal counters, incl. an ef
     far above the number of nodes."""
     metric, dims, m, efc, n, levels, ef, nq = case
