@@ -208,8 +208,8 @@ static const Conn *search_conn(void)
 	return &g_conn[(unsigned) getpid() % (unsigned) g_nconn];
 }
 
-/* ---- one request ------------------------------------------------------------------------------------------------ */
-static PgembIpcSlot *claim_slot(const Conn *c)
+/* ---- one request: claim_slot, fill, submit_wait, read the result, end_request ------------------------------------- */
+static PgembIpcSlot *claim_slot(const Conn *c, uint32_t op, uint64_t index_key)
 {
 	const uint32_t n = c->hdr->n_slots;
 	uint32_t	   start = ((uint32_t) getpid() * 2654435761u) % n;
@@ -223,9 +223,11 @@ static PgembIpcSlot *claim_slot(const Conn *c)
 			if (ld(&s->state) == PGEMB_SLOT_FREE &&
 				__atomic_compare_exchange_n(&s->state, &expect, PGEMB_SLOT_CLAIMED, 0, __ATOMIC_ACQ_REL, __ATOMIC_RELAXED))
 			{
-				/* ownership: the previous user cleared owner_pid before it freed the slot (release_slot, the sidecar's own frees), so
+				/* ownership: the previous user cleared owner_pid before it freed the slot (end_request, the sidecar's own frees), so
 				 * between the CAS above and this store the sidecar's reclaim() sees pid 0 and leaves the slot alone */
 				__atomic_store_n(&s->owner_pid, (int32_t) getpid(), __ATOMIC_RELEASE);
+				s->op = op;
+				s->index_key = index_key;
 				s->status = 0;
 				s->n_out = 0;
 				s->a0 = s->a1 = s->a2 = s->a3 = 0;
@@ -296,14 +298,17 @@ static int submit_wait(const Conn *c, PgembIpcSlot *s)
 }
 
 static int interrupted(int rc) { return rc == PGEMB_CLIENT_INTERRUPTED || rc == PGEMB_INTERRUPTED_COMPLETED; }
-/* give a slot back after submit_wait() -- unless the request was abandoned: then the slot is not ours any more */
-static void release_slot(PgembIpcSlot *s, int rc)
+/* give a slot back after submit_wait() -- unless the request was abandoned: then the slot is not ours any more -- and
+ * return the request's status, with either kind of interruption reported as PGEMB_CLIENT_INTERRUPTED */
+static int end_request(PgembIpcSlot *s, int rc)
 {
-	if (!interrupted(rc) && ld(&s->state) == PGEMB_SLOT_DONE)
+	if (interrupted(rc)) return PGEMB_CLIENT_INTERRUPTED;
+	if (ld(&s->state) == PGEMB_SLOT_DONE)
 	{
 		__atomic_store_n(&s->owner_pid, 0, __ATOMIC_RELEASE); /* never leave a stale pid on a FREE slot (see claim_slot) */
 		st(&s->state, PGEMB_SLOT_FREE);
 	}
+	return rc;
 }
 
 /* the bulk area is one request's at a time */
@@ -325,24 +330,23 @@ static int bulk_acquire(const Conn *c)
 }
 static void bulk_release(const Conn *c) { st(&c->hdr->bulk_lock, 0); }
 
-/* a request without payload on one connection (never re-maps: callers may hold pointers into the segment) */
+/* a request without payload on one connection (never re-maps: callers may hold pointers into the segment).  Returns
+ * submit_wait()'s status: a bulk request interrupted after it completed (PGEMB_INTERRUPTED_COMPLETED) leaves the bulk area
+ * to its caller, one still pending (PGEMB_CLIENT_INTERRUPTED) to the sidecar */
 static int do_request(const Conn *c, PgembClientIndex *h, uint32_t op, uint64_t a0, uint64_t a1, uint64_t a2, uint64_t a3, uint64_t *r0,
 					  uint64_t *r1, uint64_t *r2)
 {
-	int			  rc;
-	PgembIpcSlot *s = claim_slot(c);
+	PgembIpcSlot *s = claim_slot(c, op, h ? h->rel_key : 0);
 	if (!s) return PGEMB_ERR_STATE;
-	s->op = op;
-	s->index_key = h ? h->rel_key : 0;
 	s->a0 = a0;
 	s->a1 = a1;
 	s->a2 = a2;
 	s->a3 = a3;
-	rc = submit_wait(c, s);
+	const int rc = submit_wait(c, s);
 	if (r0) *r0 = s->a0;
 	if (r1) *r1 = s->a1;
 	if (r2) *r2 = s->a2;
-	release_slot(s, rc);
+	end_request(s, rc);
 	return rc;
 }
 
@@ -371,10 +375,8 @@ int pgemb_client_attach(PgembClientIndex *h, size_t capacity, size_t *size_out, 
 	for (int i = 0; i < g_nconn && rc == PGEMB_OK; i++)
 	{
 		const Conn	 *c = &g_conn[i];
-		PgembIpcSlot *s = claim_slot(c);
+		PgembIpcSlot *s = claim_slot(c, PGEMB_OP_ATTACH, h->rel_key);
 		if (!s) return PGEMB_ERR_STATE;
-		s->op = PGEMB_OP_ATTACH;
-		s->index_key = h->rel_key;
 		s->a0 = capacity;
 		memcpy(slot_vec(s), &h->meta, sizeof(HnswMetadata));
 		rc = submit_wait(c, s);
@@ -385,9 +387,9 @@ int pgemb_client_attach(PgembClientIndex *h, size_t capacity, size_t *size_out, 
 			if (size_out && (i == 0 || (size_t) s->a1 < *size_out)) *size_out = (size_t) s->a1;
 			if (capacity_out && (i == 0 || (size_t) s->a2 < *capacity_out)) *capacity_out = (size_t) s->a2;
 		}
-		release_slot(s, rc);
+		rc = end_request(s, rc);
 	}
-	return interrupted(rc) ? PGEMB_CLIENT_INTERRUPTED : rc;
+	return rc;
 }
 
 /* move `n` items of `item_bytes` through one connection's bulk area in chunks; to_server: copy in before each request, else copy out after */
@@ -481,58 +483,38 @@ int pgemb_client_build(PgembClientIndex *h, size_t first, size_t n, size_t batch
 	return rc;
 }
 
-int pgemb_client_stats(uint64_t *n_batches, uint64_t *n_searches, uint64_t *max_batch)
-{
-	const int rc = ensure_connected();
-	if (rc) return rc;
-	uint64_t b = 0, s = 0, m = 0;
-	for (int i = 0; i < g_nconn; i++)
-	{
-		b += __atomic_load_n(&g_conn[i].hdr->n_batches, __ATOMIC_RELAXED);
-		s += __atomic_load_n(&g_conn[i].hdr->n_searches, __ATOMIC_RELAXED);
-		const uint64_t mi = __atomic_load_n(&g_conn[i].hdr->max_batch, __ATOMIC_RELAXED);
-		if (mi > m) m = mi;
-	}
-	if (n_batches) *n_batches = b;
-	if (n_searches) *n_searches = s;
-	if (max_batch) *max_batch = m;
-	return PGEMB_OK;
-}
-
-int pgemb_client_scan_stats(uint64_t *n_calls, uint64_t *n_scans, uint64_t *max_batch)
+/* one counter triple (calls, requests served, largest batch; ipc.h) at byte `off` of the header, over the connected replicas:
+ * the first two summed, the largest batch the maximum */
+static int replica_stats(size_t off, uint64_t *calls, uint64_t *served, uint64_t *largest)
 {
 	const int rc = ensure_connected();
 	if (rc) return rc;
 	uint64_t c = 0, s = 0, m = 0;
 	for (int i = 0; i < g_nconn; i++)
 	{
-		c += __atomic_load_n(&g_conn[i].hdr->n_scan_calls, __ATOMIC_RELAXED);
-		s += __atomic_load_n(&g_conn[i].hdr->n_scans, __ATOMIC_RELAXED);
-		const uint64_t mi = __atomic_load_n(&g_conn[i].hdr->max_scan_batch, __ATOMIC_RELAXED);
+		const uint64_t *t = (const uint64_t *) ((const unsigned char *) g_conn[i].hdr + off);
+		c += __atomic_load_n(&t[0], __ATOMIC_RELAXED);
+		s += __atomic_load_n(&t[1], __ATOMIC_RELAXED);
+		const uint64_t mi = __atomic_load_n(&t[2], __ATOMIC_RELAXED);
 		if (mi > m) m = mi;
 	}
-	if (n_calls) *n_calls = c;
-	if (n_scans) *n_scans = s;
-	if (max_batch) *max_batch = m;
+	if (calls) *calls = c;
+	if (served) *served = s;
+	if (largest) *largest = m;
 	return PGEMB_OK;
 }
 
+int pgemb_client_stats(uint64_t *n_batches, uint64_t *n_searches, uint64_t *max_batch)
+{
+	return replica_stats(offsetof(PgembIpcHeader, n_batches), n_batches, n_searches, max_batch);
+}
+int pgemb_client_scan_stats(uint64_t *n_calls, uint64_t *n_scans, uint64_t *max_batch)
+{
+	return replica_stats(offsetof(PgembIpcHeader, n_scan_calls), n_calls, n_scans, max_batch);
+}
 int pgemb_client_dist_stats(uint64_t *n_calls, uint64_t *n_dists, uint64_t *max_batch)
 {
-	const int rc = ensure_connected();
-	if (rc) return rc;
-	uint64_t c = 0, d = 0, m = 0;
-	for (int i = 0; i < g_nconn; i++)
-	{
-		c += __atomic_load_n(&g_conn[i].hdr->n_dist_calls, __ATOMIC_RELAXED);
-		d += __atomic_load_n(&g_conn[i].hdr->n_dists, __ATOMIC_RELAXED);
-		const uint64_t mi = __atomic_load_n(&g_conn[i].hdr->max_dist_batch, __ATOMIC_RELAXED);
-		if (mi > m) m = mi;
-	}
-	if (n_calls) *n_calls = c;
-	if (n_dists) *n_dists = d;
-	if (max_batch) *max_batch = m;
-	return PGEMB_OK;
+	return replica_stats(offsetof(PgembIpcHeader, n_dist_calls), n_calls, n_dists, max_batch);
 }
 
 /* ---- the index-less scan (embedding.c:1022-1062 per row + the executor's sort; knn.out:63-91) ------------------------- */
@@ -557,10 +539,8 @@ int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, 
 		set_err("pgemb_client_scan_topk: dims outside the sidecar's limits");
 		return PGEMB_ERR_ARG;
 	}
-	PgembIpcSlot *s = claim_slot(c);
+	PgembIpcSlot *s = claim_slot(c, PGEMB_OP_SCAN, h->rel_key);
 	if (!s) return PGEMB_ERR_STATE;
-	s->op = PGEMB_OP_SCAN;
-	s->index_key = h->rel_key;
 	s->a0 = k;
 	memcpy(slot_vec(s), query, h->meta.dim * sizeof(coord_t));
 	rc = submit_wait(c, s);
@@ -579,8 +559,7 @@ int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, 
 			rc = PGEMB_ERR_STATE;
 		}
 	}
-	release_slot(s, rc);
-	return interrupted(rc) ? PGEMB_CLIENT_INTERRUPTED : rc;
+	return end_request(s, rc);
 }
 
 int pgemb_client_shutdown_server(void) { return simple_request(1, NULL, PGEMB_OP_SHUTDOWN, 0, 0, 0, 0, NULL, NULL, NULL); }
@@ -600,26 +579,22 @@ bool hnsw_search(HnswMetadata *meta, const coord_t *point, size_t *n_results, la
 	}
 	label_t *buf = (label_t *) malloc(ef * sizeof(label_t));
 	if (!buf) return false;
-	PgembIpcSlot *s = claim_slot(c);
-	if (!s)
+	PgembIpcSlot *s = claim_slot(c, PGEMB_OP_SEARCH, h->rel_key);
+	bool		  ok = false;
+	if (s)
 	{
-		free(buf);
-		return false;
+		s->ef = (uint32_t) ef;
+		memcpy(slot_vec(s), point, meta->dim * sizeof(coord_t));
+		const int rc = submit_wait(c, s);
+		if (rc == PGEMB_OK && s->n_out >= 0 && (size_t) s->n_out <= ef)
+		{
+			memcpy(buf, slot_labels(c, s), (size_t) s->n_out * sizeof(label_t));
+			*n_results = (size_t) s->n_out;
+			*results = buf;
+			ok = true;
+		}
+		end_request(s, rc);
 	}
-	s->op = PGEMB_OP_SEARCH;
-	s->index_key = h->rel_key;
-	s->ef = (uint32_t) ef;
-	memcpy(slot_vec(s), point, meta->dim * sizeof(coord_t));
-	const int rc = submit_wait(c, s);
-	bool	  ok = false;
-	if (rc == PGEMB_OK && s->n_out >= 0 && (size_t) s->n_out <= ef)
-	{
-		memcpy(buf, slot_labels(c, s), (size_t) s->n_out * sizeof(label_t));
-		*n_results = (size_t) s->n_out;
-		*results = buf;
-		ok = true;
-	}
-	release_slot(s, rc);
 	if (!ok) free(buf);
 	return ok;
 }
@@ -643,10 +618,8 @@ dist_t hnsw_dist_func(dist_func_t dist, coord_t const *ax, coord_t const *bx, si
 	if (!ax || !bx || ensure_connected() != PGEMB_OK) return NAN;
 	const Conn *c = search_conn();
 	if (dim < 1 || dim > c->hdr->max_dim) return NAN;
-	PgembIpcSlot *s = claim_slot(c);
+	PgembIpcSlot *s = claim_slot(c, PGEMB_OP_DIST, 0);
 	if (!s) return NAN;
-	s->op = PGEMB_OP_DIST;
-	s->index_key = 0;
 	s->a0 = dim;
 	s->a1 = (uint64_t) dist;
 	memcpy(slot_vec(s), ax, dim * sizeof(coord_t));
@@ -658,7 +631,7 @@ dist_t hnsw_dist_func(dist_func_t dist, coord_t const *ax, coord_t const *bx, si
 		const uint32_t bits = (uint32_t) s->a2;
 		memcpy(&out, &bits, 4);
 	}
-	release_slot(s, rc);
+	end_request(s, rc);
 	return out;
 }
 

@@ -31,6 +31,7 @@
 #include <cstring>
 #include <map>
 #include <string>
+#include <tuple>
 #include <unordered_map>
 #include <vector>
 
@@ -104,10 +105,8 @@ double now_s()
 volatile sig_atomic_t g_stop = 0;
 void				  on_signal(int) { g_stop = 1; }
 
-struct Mirror
-{
-	PgembHostIndex host;  // {meta, dev}: what the reference-shaped entry points down-cast their HnswMetadata* to
-};
+// A batched group: (PGEMB_OP_SEARCH, relation, ef), (PGEMB_OP_SCAN, relation, k) or (PGEMB_OP_DIST, metric, dim)
+using GroupKey = std::tuple<uint32_t, uint64_t, uint64_t>;
 
 struct Server
 {
@@ -122,7 +121,7 @@ struct Server
 	double			last_service_s = 0.0;	// duration of the previous round's launches
 	size_t			carry = 0;				// searches that queued up while the current round's launches ran
 	bool			carry_counted = false;
-	std::unordered_map<uint64_t, Mirror> mirrors;
+	std::unordered_map<uint64_t, PgembHostIndex> mirrors;  // {meta, dev}: what the reference-shaped entry points down-cast their HnswMetadata* to
 	// per-batch scratch
 	std::vector<float>	  qbuf;
 	std::vector<float>	  bbuf;	 // second vectors of the distance pairs
@@ -175,7 +174,7 @@ struct Server
 	}
 	void finish_api(PgembIpcSlot *s, pgemb_status status) { finish(s, status, status == PGEMB_OK ? nullptr : api.last_error()); }
 
-	Mirror *find(PgembIpcSlot *s)
+	PgembHostIndex *find(PgembIpcSlot *s)
 	{
 		auto it = mirrors.find(s->index_key);
 		if (it == mirrors.end())
@@ -199,6 +198,20 @@ struct Server
 	// ---- everything except searches, scans and distances: one at a time, in slot order ----------------------------
 	void run_control(PgembIpcSlot *s)
 	{
+		PgembHostIndex *m = nullptr;
+		switch (s->op)
+		{
+			// the requests on an attached mirror
+			case PGEMB_OP_APPEND_RECORDS:
+			case PGEMB_OP_BIND:
+			case PGEMB_OP_GET_LINKS:
+			case PGEMB_OP_EXPORT_RECORDS:
+			case PGEMB_OP_SET_LABELS:
+			case PGEMB_OP_TRUNCATE:
+			case PGEMB_OP_SIZE:
+			case PGEMB_OP_BUILD:
+				if (!(m = find(s))) return;
+		}
 		switch (s->op)
 		{
 			case PGEMB_OP_PING: finish(s, PGEMB_OK, nullptr); return;
@@ -210,8 +223,8 @@ struct Server
 				if (it != mirrors.end())
 				{
 					// the reference checks {dims, maxM} of an existing index against the options (embedding.c:594-602)
-					const HnswMetadata &m = it->second.host.meta;
-					if (m.dim != meta.dim || m.maxM != meta.maxM || m.dist_func != meta.dist_func)
+					const HnswMetadata &have = it->second.meta;
+					if (have.dim != meta.dim || have.maxM != meta.maxM || have.dist_func != meta.dist_func)
 					{
 						finish(s, PGEMB_ERR_ARG, "attach: dims / maxM / distance function differ from the attached index");
 						return;
@@ -224,123 +237,91 @@ struct Server
 						finish(s, PGEMB_ERR_ARG, "attach: dims outside the sidecar's --max-dim");
 						return;
 					}
-					Mirror m;
-					m.host.meta = meta;
-					m.host.dev = nullptr;
-					const pgemb_status r = api.index_create(&meta, (size_t) s->a0, device, &m.host.dev);
+					PgembHostIndex created = {meta, nullptr};
+					const pgemb_status r = api.index_create(&meta, (size_t) s->a0, device, &created.dev);
 					if (r != PGEMB_OK)
 					{
 						finish_api(s, r);
 						return;
 					}
-					it = mirrors.emplace(s->index_key, m).first;
+					it = mirrors.emplace(s->index_key, created).first;
 				}
-				if ((size_t) s->a0 > api.index_capacity(it->second.host.dev))
+				if ((size_t) s->a0 > api.index_capacity(it->second.dev))
 				{
 					// the relation has grown beyond the mirror: make room (ids and contents are kept)
-					const pgemb_status r = api.reserve(it->second.host.dev, (size_t) s->a0);
+					const pgemb_status r = api.reserve(it->second.dev, (size_t) s->a0);
 					if (r != PGEMB_OK)
 					{
 						finish_api(s, r);
 						return;
 					}
 				}
-				s->a1 = api.index_size(it->second.host.dev);
-				s->a2 = api.index_capacity(it->second.host.dev);
+				s->a1 = api.index_size(it->second.dev);
+				s->a2 = api.index_capacity(it->second.dev);
 				finish(s, PGEMB_OK, nullptr);
 				return;
 			}
 			case PGEMB_OP_APPEND_RECORDS:
 			{
-				Mirror *m = find(s);
-				if (!m) return;
 				if (!bulk_owned_by(s, (size_t) s->a0 * (size_t) s->a1)) return;
+				// a relation grows page by page (embedding.c:636-691): the mirror grows with it, doubling
+				const size_t have = api.index_size(m->dev), cap = api.index_capacity(m->dev), need = have + (size_t) s->a0;
+				if (need > cap)
 				{
-					// a relation grows page by page (embedding.c:636-691): the mirror grows with it, doubling
-					const size_t have = api.index_size(m->host.dev), cap = api.index_capacity(m->host.dev), need = have + (size_t) s->a0;
-					if (need > cap)
+					const pgemb_status r = api.reserve(m->dev, need > 2 * cap ? need : 2 * cap);
+					if (r != PGEMB_OK)
 					{
-						const pgemb_status r = api.reserve(m->host.dev, need > 2 * cap ? need : 2 * cap);
-						if (r != PGEMB_OK)
-						{
-							finish_api(s, r);
-							return;
-						}
+						finish_api(s, r);
+						return;
 					}
 				}
-				finish_api(s, api.append_records(m->host.dev, (size_t) s->a0, bulk(), (size_t) s->a1));
+				finish_api(s, api.append_records(m->dev, (size_t) s->a0, bulk(), (size_t) s->a1));
 				return;
 			}
 			case PGEMB_OP_BIND:
 			{
-				Mirror *m = find(s);
-				if (!m) return;
-				m->host.meta.efConstruction = (size_t) s->a1;  // re-read on every call, like the library does for a local caller
-				const bool ok = api.bind_point(&m->host.meta, nullptr, (idx_t) s->a0);
+				m->meta.efConstruction = (size_t) s->a1;  // re-read on every call, like the library does for a local caller
+				const bool ok = api.bind_point(&m->meta, nullptr, (idx_t) s->a0);
 				finish(s, ok ? PGEMB_OK : PGEMB_ERR_STATE, ok ? nullptr : api.last_error());
 				return;
 			}
 			case PGEMB_OP_GET_LINKS:
-			{
-				Mirror *m = find(s);
-				if (!m) return;
-				if (!bulk_owned_by(s, (size_t) s->a1 * (m->host.meta.maxM + 1) * sizeof(idx_t))) return;
-				finish_api(s, api.get_links(m->host.dev, (size_t) s->a0, (size_t) s->a1, reinterpret_cast<idx_t *>(bulk())));
+				if (!bulk_owned_by(s, (size_t) s->a1 * (m->meta.maxM + 1) * sizeof(idx_t))) return;
+				finish_api(s, api.get_links(m->dev, (size_t) s->a0, (size_t) s->a1, reinterpret_cast<idx_t *>(bulk())));
 				return;
-			}
 			case PGEMB_OP_EXPORT_RECORDS:
-			{
-				Mirror *m = find(s);
-				if (!m) return;
 				if (!bulk_owned_by(s, (size_t) s->a1 * (size_t) s->a2)) return;
-				finish_api(s, api.export_records(m->host.dev, (size_t) s->a0, (size_t) s->a1, bulk(), (size_t) s->a2));
+				finish_api(s, api.export_records(m->dev, (size_t) s->a0, (size_t) s->a1, bulk(), (size_t) s->a2));
 				return;
-			}
 			case PGEMB_OP_SET_LABELS:
-			{
-				Mirror *m = find(s);
-				if (!m) return;
 				if (!bulk_owned_by(s, (size_t) s->a1 * sizeof(label_t))) return;
-				finish_api(s, api.set_labels(m->host.dev, (size_t) s->a0, (size_t) s->a1, reinterpret_cast<const label_t *>(bulk())));
+				finish_api(s, api.set_labels(m->dev, (size_t) s->a0, (size_t) s->a1, reinterpret_cast<const label_t *>(bulk())));
 				return;
-			}
-			case PGEMB_OP_TRUNCATE:
-			{
-				Mirror *m = find(s);
-				if (!m) return;
-				finish_api(s, api.truncate(m->host.dev));
-				return;
-			}
+			case PGEMB_OP_TRUNCATE: finish_api(s, api.truncate(m->dev)); return;
 			case PGEMB_OP_DROP:
 			{
 				auto it = mirrors.find(s->index_key);
 				if (it != mirrors.end())
 				{
-					api.index_destroy(it->second.host.dev);
+					api.index_destroy(it->second.dev);
 					mirrors.erase(it);
 				}
 				finish(s, PGEMB_OK, nullptr);
 				return;
 			}
 			case PGEMB_OP_SIZE:
-			{
-				Mirror *m = find(s);
-				if (!m) return;
-				s->a0 = api.index_size(m->host.dev);
-				s->a1 = api.index_capacity(m->host.dev);
+				s->a0 = api.index_size(m->dev);
+				s->a1 = api.index_capacity(m->dev);
 				finish(s, PGEMB_OK, nullptr);
 				return;
-			}
 			case PGEMB_OP_BUILD:
 			{
-				Mirror *m = find(s);
-				if (!m) return;
 				double		 sec = 0.0;
 				pgemb_status r;
 				if (s->a3)
-					r = api.build_exact(m->host.dev, (size_t) s->a0, (size_t) s->a1, (size_t) s->a2, &sec, nullptr);
+					r = api.build_exact(m->dev, (size_t) s->a0, (size_t) s->a1, (size_t) s->a2, &sec, nullptr);
 				else
-					r = api.build_bulk(m->host.dev, (size_t) s->a0, (size_t) s->a1, (size_t) s->a2, &sec);
+					r = api.build_bulk(m->dev, (size_t) s->a0, (size_t) s->a1, (size_t) s->a2, &sec);
 				memcpy(&s->a2, &sec, sizeof(sec));
 				finish_api(s, r);
 				return;
@@ -353,131 +334,94 @@ struct Server
 		}
 	}
 
-	// ---- searches: all requests of one (relation, ef) that are pending now -> one launch -------------------------------
-	void run_searches(std::vector<PgembIpcSlot *> &group)
+	// ---- batched requests: all pending requests of one group -> one library call per max_batch --------------------
+	// Searches launch pgemb_search_batch, scans pgemb_scan_topk and distances pgemb_dist_batch.  Scans are grouped by k, not
+	// folded into the largest k of the relation: a query's re-scoring work grows with k (DESIGN.md section 6).  Every
+	// distance pair is independent and gets the bits of a one-pair call: the same dist_pairs_kernel evaluates each pair alone.
+	void run_group(const GroupKey &key, const std::vector<PgembIpcSlot *> &group)
 	{
-		PgembIpcSlot *s0 = group[0];
-		auto		  it = mirrors.find(s0->index_key);
-		const size_t  ef = s0->ef;
-		if (it == mirrors.end() || ef < 1 || ef > hdr->max_ef)
-		{
-			for (PgembIpcSlot *s : group)
-				finish(s, PGEMB_ERR_ARG, it == mirrors.end() ? "no device index attached for this relation key" : "efSearch outside the sidecar's --max-ef");
-			return;
-		}
-		Mirror		&m = it->second;
-		const size_t dim = m.host.meta.dim;
-		for (size_t lo = 0; lo < group.size(); lo += max_batch)
-		{
-			const size_t nq = std::min(max_batch, group.size() - lo);
-			qbuf.resize(nq * dim);
-			lbuf.resize(nq * ef);
-			nbuf.assign(nq, 0);
-			for (size_t i = 0; i < nq; i++) memcpy(&qbuf[i * dim], slot_vec(group[lo + i]), dim * sizeof(float));
-			const pgemb_status r = api.search_batch(m.host.dev, nq, qbuf.data(), ef, lbuf.data(), nullptr, nullptr, nbuf.data(), nullptr);
-			if (!carry_counted)
-			{
-				// who queued up while the launch ran (BEFORE any result of this round is published: a caller that gets its
-				// result resubmits at once and would be counted twice)
-				carry_counted = true;
-				for (uint32_t i = 0; i < hdr->n_slots; i++)
-				{
-					const PgembIpcSlot *c = slot(i);
-					if (ld(&c->state) == PGEMB_SLOT_READY && c->op == PGEMB_OP_SEARCH) carry++;
-				}
-			}
-			hdr->n_batches += 1;
-			hdr->n_searches += nq;
-			if (nq > hdr->max_batch) hdr->max_batch = nq;
-			for (size_t i = 0; i < nq; i++)
-			{
-				PgembIpcSlot *s = group[lo + i];
-				if (r == PGEMB_OK)
-				{
-					const int32_t n = nbuf[i];
-					s->n_out = n;
-					memcpy(slot_labels(s), &lbuf[i * ef], (size_t) (n > 0 ? n : 0) * sizeof(label_t));
-				}
-				finish_api(s, r);
-			}
-		}
-	}
-
-	// ---- index-less scans: all requests of one (relation, k) that are pending now -> one pgemb_scan_topk per max_batch ----
-	// Grouped by k, not folded into the largest k of the relation: a query's re-scoring work grows with k (DESIGN.md section 6).
-	void run_scans(std::vector<PgembIpcSlot *> &group)
-	{
-		PgembIpcSlot *s0 = group[0];
-		auto		  it = mirrors.find(s0->index_key);
-		const size_t  k = (size_t) s0->a0;
-		if (it == mirrors.end() || k < 1 || k > std::min<size_t>(4096, hdr->max_ef))
-		{
-			for (PgembIpcSlot *s : group)
-				finish(s, PGEMB_ERR_ARG, it == mirrors.end() ? "no device index attached for this relation key" : "scan: k outside 1 .. min(4096, the sidecar's --max-ef)");
-			return;
-		}
-		Mirror		&m = it->second;
-		const size_t dim = m.host.meta.dim;
-		for (size_t lo = 0; lo < group.size(); lo += max_batch)
-		{
-			const size_t nq = std::min(max_batch, group.size() - lo);
-			qbuf.resize(nq * dim);
-			lbuf.resize(nq * k);
-			dbuf.resize(nq * k);
-			nbuf.assign(nq, 0);
-			for (size_t i = 0; i < nq; i++) memcpy(&qbuf[i * dim], slot_vec(group[lo + i]), dim * sizeof(float));
-			const pgemb_status r = api.scan_topk(m.host.dev, nq, qbuf.data(), k, lbuf.data(), dbuf.data(), nbuf.data());
-			hdr->n_scan_calls += 1;
-			hdr->n_scans += nq;
-			if (nq > hdr->max_scan_batch) hdr->max_scan_batch = nq;
-			for (size_t i = 0; i < nq; i++)
-			{
-				PgembIpcSlot *s = group[lo + i];
-				if (r == PGEMB_OK)
-				{
-					const size_t n = (size_t) (nbuf[i] > 0 ? nbuf[i] : 0);
-					s->n_out = nbuf[i];
-					memcpy(slot_labels(s), &lbuf[i * k], n * sizeof(label_t));
-					memcpy(slot_dists(s), &dbuf[i * k], n * sizeof(float));
-				}
-				finish_api(s, r);
-			}
-		}
-	}
-
-	// ---- distances (hnsw_dist_func): all pending pairs of one (metric, dim) -> one pgemb_dist_batch per max_batch ----
-	// Every pair is independent and gets the bits of a one-pair call: the same dist_pairs_kernel evaluates each pair alone.
-	void run_dists(uint64_t metric, uint64_t dim, std::vector<PgembIpcSlot *> &group)
-	{
-		if (dim < 1 || dim > hdr->max_dim || metric > 2)
+		const auto [op, g, k] = key;  // g: relation key (search, scan) or metric (distance); k: ef, k or dim
+		PgembHostIndex *m = nullptr;
+		const char	   *bad = nullptr;
+		if (op == PGEMB_OP_DIST)
 		{
 			// the whole group shares the bad (metric, dim): each request fails by itself, the other groups are not affected
-			for (PgembIpcSlot *s : group) finish(s, PGEMB_ERR_ARG, "dist: bad dimension or metric");
+			if (k < 1 || k > hdr->max_dim || g > 2) bad = "dist: bad dimension or metric";
+		}
+		else if (auto it = mirrors.find(g); it == mirrors.end())
+			bad = "no device index attached for this relation key";
+		else if (op == PGEMB_OP_SEARCH && (k < 1 || k > hdr->max_ef))
+			bad = "efSearch outside the sidecar's --max-ef";
+		else if (op == PGEMB_OP_SCAN && (k < 1 || k > std::min<size_t>(4096, hdr->max_ef)))
+			bad = "scan: k outside 1 .. min(4096, the sidecar's --max-ef)";
+		else
+			m = &it->second;
+		if (bad)
+		{
+			for (PgembIpcSlot *s : group) finish(s, PGEMB_ERR_ARG, bad);
 			return;
 		}
+		const size_t dim = m ? m->meta.dim : k;
 		for (size_t lo = 0; lo < group.size(); lo += max_batch)
 		{
-			const size_t n = std::min(max_batch, group.size() - lo);
-			qbuf.resize(n * dim);
-			bbuf.resize(n * dim);
-			dbuf.resize(n);
-			for (size_t i = 0; i < n; i++)
+			const size_t nq = std::min(max_batch, group.size() - lo);
+			auto		 count = [nq](uint64_t &calls, uint64_t &served, uint64_t &largest) {
+				calls += 1;
+				served += nq;
+				if (nq > largest) largest = nq;
+			};
+			qbuf.resize(nq * dim);
+			for (size_t i = 0; i < nq; i++) memcpy(&qbuf[i * dim], slot_vec(group[lo + i]), dim * sizeof(float));
+			pgemb_status r;
+			if (op == PGEMB_OP_SEARCH)
 			{
-				memcpy(&qbuf[i * dim], slot_vec(group[lo + i]), dim * sizeof(float));
-				memcpy(&bbuf[i * dim], slot_vec(group[lo + i]) + hdr->max_dim, dim * sizeof(float));
+				lbuf.resize(nq * k);
+				nbuf.assign(nq, 0);
+				r = api.search_batch(m->dev, nq, qbuf.data(), k, lbuf.data(), nullptr, nullptr, nbuf.data(), nullptr);
+				if (!carry_counted)
+				{
+					// who queued up while the launch ran (BEFORE any result of this round is published: a caller that gets its
+					// result resubmits at once and would be counted twice)
+					carry_counted = true;
+					for (uint32_t i = 0; i < hdr->n_slots; i++)
+					{
+						const PgembIpcSlot *c = slot(i);
+						if (ld(&c->state) == PGEMB_SLOT_READY && c->op == PGEMB_OP_SEARCH) carry++;
+					}
+				}
+				count(hdr->n_batches, hdr->n_searches, hdr->max_batch);
 			}
-			const pgemb_status r = api.dist_batch((dist_func_t) metric, (size_t) dim, n, qbuf.data(), 0, bbuf.data(), dbuf.data());
-			hdr->n_dist_calls += 1;
-			hdr->n_dists += n;
-			if (n > hdr->max_dist_batch) hdr->max_dist_batch = n;
-			for (size_t i = 0; i < n; i++)
+			else if (op == PGEMB_OP_SCAN)
+			{
+				lbuf.resize(nq * k);
+				dbuf.resize(nq * k);
+				nbuf.assign(nq, 0);
+				r = api.scan_topk(m->dev, nq, qbuf.data(), k, lbuf.data(), dbuf.data(), nbuf.data());
+				count(hdr->n_scan_calls, hdr->n_scans, hdr->max_scan_batch);
+			}
+			else
+			{
+				bbuf.resize(nq * dim);
+				dbuf.resize(nq);
+				for (size_t i = 0; i < nq; i++) memcpy(&bbuf[i * dim], slot_vec(group[lo + i]) + hdr->max_dim, dim * sizeof(float));
+				r = api.dist_batch((dist_func_t) g, dim, nq, qbuf.data(), 0, bbuf.data(), dbuf.data());
+				count(hdr->n_dist_calls, hdr->n_dists, hdr->max_dist_batch);
+			}
+			for (size_t i = 0; i < nq; i++)
 			{
 				PgembIpcSlot *s = group[lo + i];
-				if (r == PGEMB_OK)
+				if (r == PGEMB_OK && op == PGEMB_OP_DIST)
 				{
 					uint32_t bits;
 					memcpy(&bits, &dbuf[i], 4);
 					s->a2 = bits;
+				}
+				else if (r == PGEMB_OK)
+				{
+					const size_t n = (size_t) (nbuf[i] > 0 ? nbuf[i] : 0);
+					s->n_out = nbuf[i];
+					memcpy(slot_labels(s), &lbuf[i * k], n * sizeof(label_t));
+					if (op == PGEMB_OP_SCAN) memcpy(slot_dists(s), &dbuf[i * k], n * sizeof(float));
 				}
 				finish_api(s, r);
 			}
@@ -488,39 +432,39 @@ struct Server
 	size_t serve_once()
 	{
 		std::vector<PgembIpcSlot *> control;
-		std::map<std::pair<uint64_t, uint32_t>, std::vector<PgembIpcSlot *>> searches;
-		std::map<std::pair<uint64_t, uint64_t>, std::vector<PgembIpcSlot *>> scans;
-		std::map<std::pair<uint64_t, uint64_t>, std::vector<PgembIpcSlot *>> dists;  // (metric, dim)
+		std::map<GroupKey, std::vector<PgembIpcSlot *>> batched;
 		size_t found = 0, nsearch = 0;
 		auto   collect = [&]() {
-			  for (uint32_t i = 0; i < hdr->n_slots; i++)
-			  {
-				  PgembIpcSlot *s = slot(i);
-				  if (ld(&s->state) != PGEMB_SLOT_READY) continue;
-				  st(&s->state, PGEMB_SLOT_BUSY);
-				  found++;
-				  if (s->op == PGEMB_OP_SEARCH)
-				  {
-					  searches[{s->index_key, s->ef}].push_back(s);
-					  nsearch++;
-				  }
-				  else if (s->op == PGEMB_OP_SCAN)
-					  scans[{s->index_key, s->a0}].push_back(s);  // not part of the searches' linger bookkeeping (nsearch / target / carry)
-				  else if (s->op == PGEMB_OP_DIST)
-					  dists[{s->a1, s->a0}].push_back(s);	 // touches no mirror, so no place in the write/search order; never lingers
-				  else
-					  control.push_back(s);
-			  }
+			for (uint32_t i = 0; i < hdr->n_slots; i++)
+			{
+				PgembIpcSlot *s = slot(i);
+				if (ld(&s->state) != PGEMB_SLOT_READY) continue;
+				st(&s->state, PGEMB_SLOT_BUSY);
+				found++;
+				if (s->op == PGEMB_OP_SEARCH)
+				{
+					batched[{s->op, s->index_key, s->ef}].push_back(s);
+					nsearch++;
+				}
+				else if (s->op == PGEMB_OP_SCAN)
+					batched[{s->op, s->index_key, s->a0}].push_back(s);  // not part of the searches' linger bookkeeping (nsearch / target / carry)
+				else if (s->op == PGEMB_OP_DIST)
+					batched[{s->op, s->a1, s->a0}].push_back(s);	 // touches no mirror, so no place in the write/search order; never lingers
+				else
+					control.push_back(s);
+			}
 		};
-		// Distances first, as soon as they are collected: a one-pair request must not wait behind the searches' launches or
-		// their linger below.  Whatever queued up while the previous pass ran is served by one call per (metric, dim).
-		auto run_pending_dists = [&]() {
-			for (auto &kv : dists) run_dists(kv.first.first, kv.first.second, kv.second);
-			dists.clear();
+		// serve every collected group of one kind, in key order
+		auto run_groups = [&](uint32_t op) {
+			const auto first = batched.lower_bound(GroupKey{op, 0, 0}), last = batched.lower_bound(GroupKey{op + 1, 0, 0});
+			for (auto it = first; it != last; ++it) run_group(it->first, it->second);
+			batched.erase(first, last);
 		};
 		collect();
 		if (found == 0) return 0;
-		run_pending_dists();
+		// Distances first, as soon as they are collected: a one-pair request must not wait behind the searches' launches or
+		// their linger below.  Whatever queued up while the previous pass ran is served by one call per (metric, dim).
+		run_groups(PGEMB_OP_DIST);
 		// Keeping the callers together.  A caller resubmits a few microseconds after it got its result, so a server that
 		// launches whatever is queued the moment it becomes free splits P steady callers into two groups that are served
 		// alternately -- each waits two launches per result.  `target` is the number of concurrent searchers the last
@@ -537,14 +481,14 @@ struct Server
 			while (nsearch < target && now_s() < until)
 			{
 				collect();
-				run_pending_dists();
+				run_groups(PGEMB_OP_DIST);
 			}
 		}
 		for (PgembIpcSlot *s : control) run_control(s);
 		const double t_run = now_s();
 		carry = 0;
 		carry_counted = false;
-		for (auto &kv : searches) run_searches(kv.second);
+		run_groups(PGEMB_OP_SEARCH);
 		if (nsearch > 0)
 		{
 			last_service_s = now_s() - t_run;
@@ -553,7 +497,7 @@ struct Server
 				FILE *f = fopen(dbg, "a");
 				if (f) { fprintf(f, "round: nsearch %zu target %zu service %.0f us\n", nsearch, target, last_service_s * 1e6); fclose(f); }
 			}
-			// carry: callers of the "other group" (counted in run_searches, before this round's results went out)
+			// carry: callers of the "other group" (counted in run_group, before this round's results went out)
 			const size_t seen = nsearch + carry, decayed = target - (target + 9) / 10;	// forget departed callers by 10 % a round
 			target = seen > decayed ? seen : decayed;
 			if (target < 1) target = 1;
@@ -562,7 +506,7 @@ struct Server
 		// Scans last: a scan sees every write whose request completed before it was submitted, as a search does.  They
 		// never linger: a scan call takes milliseconds, and the next batch queues up by itself while it runs.  A scan and a
 		// search of the same mirror never run at the same time (the index's staging buffers and workspace are shared).
-		for (auto &kv : scans) run_scans(kv.second);
+		run_groups(PGEMB_OP_SCAN);
 		return found;
 	}
 
@@ -770,7 +714,7 @@ int main(int argc, char **argv)
 		const uint32_t stt = ld(&s->state);
 		if (stt == PGEMB_SLOT_READY || stt == PGEMB_SLOT_BUSY) srv.finish(s, PGEMB_ERR_STATE, "sidecar is shutting down");
 	}
-	for (auto &kv : srv.mirrors) srv.api.index_destroy(kv.second.host.dev);
+	for (auto &kv : srv.mirrors) srv.api.index_destroy(kv.second.dev);
 	shm_unlink(shm_name.c_str());
 	munmap(mem, bytes);
 	fprintf(stderr, "pgemb_sidecar: stopped\n");

@@ -119,31 +119,48 @@ class RawSegment:
     while no other process claims slots (the backends of a test are parked at their start line), so plain stores in the
     protocol's order are enough."""
 
+    VEC_OFF = 240                                                                     # pgemb_ipc_payload_vec_off()
+
     def __init__(self, name):
         self.f = open("/dev/shm" + name, "r+b")
         self.m = mmap.mmap(self.f.fileno(), 0)
-        self.n_slots, self.max_dim = struct.unpack_from("<II", self.m, 8)
+        self.n_slots, self.max_dim, self.max_ef = struct.unpack_from("<III", self.m, 8)
         self.stride, self.slots_off = struct.unpack_from("<I", self.m, 20)[0], struct.unpack_from("<Q", self.m, 24)[0]
+        self.labels_off = self.VEC_OFF + (2 * self.max_dim * 4 + 15) // 16 * 16
+        self.dists_off = self.labels_off + self.max_ef * 8
 
     def _off(self, i):
         return self.slots_off + i * self.stride
 
-    def submit_dist(self, dim, metric):
-        """Publish one PGEMB_OP_DIST request (a0 = dim, a1 = metric, zero vectors); returns its slot."""
+    def submit(self, op, index_key=0, a=(0, 0, 0, 0), ef=0, vec=None):
+        """Publish one request: op, index_key, a0..a3, ef and, unless None, `vec` (float32) at the start of the payload;
+        returns its slot."""
         for i in range(self.n_slots):
             o = self._off(i)
             if struct.unpack_from("<I", self.m, o)[0] != SLOT_FREE:
                 continue
-            struct.pack_into("<IIii", self.m, o, 1, OP_DIST, 0, os.getpid())        # CLAIMED, owner = this process
-            struct.pack_into("<QQQQQ", self.m, o + 16, 0, dim, metric, 0, 0)          # index_key, a0..a3
-            struct.pack_into("<Ii", self.m, o + 56, 0, 0)
+            struct.pack_into("<IIii", self.m, o, 1, op, 0, os.getpid())             # CLAIMED, owner = this process
+            struct.pack_into("<QQQQQ", self.m, o + 16, index_key, *a)                 # index_key, a0..a3
+            struct.pack_into("<Ii", self.m, o + 56, ef, 0)
             struct.pack_into("<I", self.m, o + 64, 0)
+            if vec is not None:
+                v = np.ascontiguousarray(vec, np.float32).tobytes()
+                self.m[o + self.VEC_OFF:o + self.VEC_OFF + len(v)] = v
             struct.pack_into("<I", self.m, o, SLOT_READY)
             return i
         raise AssertionError("no free slot")
 
+    def submit_dist(self, dim, metric):
+        """Publish one PGEMB_OP_DIST request (a0 = dim, a1 = metric, zero vectors); returns its slot."""
+        return self.submit(OP_DIST, a=(dim, metric, 0, 0))
+
     def wait(self, i, timeout_s=60.0):
         """(status, message) of slot i once DONE; the slot is given back."""
+        return self.wait_result(i, timeout_s)[:2]
+
+    def wait_result(self, i, timeout_s=60.0):
+        """(status, message, {"n_out", "a2", "labels", "dists"}) of slot i once DONE, the labels and distance bits of its
+        first n_out results read as a search or scan result; the slot is given back."""
         o = self._off(i)
         deadline = time.time() + timeout_s
         while struct.unpack_from("<I", self.m, o)[0] != SLOT_DONE:
@@ -151,9 +168,14 @@ class RawSegment:
             time.sleep(0.002)
         status = struct.unpack_from("<i", self.m, o + 8)[0]
         msg = bytes(self.m[o + 68:o + 68 + 164]).split(b"\0")[0].decode()
+        n = struct.unpack_from("<i", self.m, o + 60)[0]
+        k = max(0, min(n, self.max_ef))
+        res = {"n_out": n, "a2": struct.unpack_from("<Q", self.m, o + 40)[0],
+               "labels": list(struct.unpack_from(f"<{k}Q", self.m, o + self.labels_off)),
+               "dists": list(struct.unpack_from(f"<{k}I", self.m, o + self.dists_off))}
         struct.pack_into("<i", self.m, o + 12, 0)                                     # FREE slots carry no pid
         struct.pack_into("<I", self.m, o, SLOT_FREE)
-        return status, msg
+        return status, msg, res
 
     def close(self):
         self.m.close()
