@@ -181,7 +181,8 @@ uint64_t pgemb_launch_count(void);
  * out[i] = dist(a[i] or a[0] if broadcast_a, b[i]). */
 pgemb_status pgemb_dist_batch(dist_func_t dist, size_t dim, size_t n, const coord_t *a, int broadcast_a,
                               const coord_t *b, dist_t *out);
-/* Distances from nq host queries to stored nodes ids[nq*k] of a device index (gather kernel K1). */
+/* Distances from nq host queries to stored nodes ids[nq*k] of a device index (gather kernel K1).
+ * out[q*k + j] is NaN where ids[q*k + j] >= the index's size (no error is raised); the other entries are unaffected. */
 pgemb_status pgemb_dist_gather(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k,
                                const idx_t *ids, dist_t *out);
 

@@ -1,6 +1,8 @@
 // Scheduler and launcher of the host SIMT emulator (see fake_cuda/cuda_runtime.h).  Test infrastructure.
 #include <cuda_runtime.h>
 #include <signal.h>
+#include <utility>
+#include <vector>
 
 namespace emu {
 
@@ -120,8 +122,15 @@ void run_warp(Warp &w)
 	tl_warp = nullptr;
 }
 
+// (threads per CTA, dynamic shared memory) of the first 4096 launches since the log was last read, and how many there
+// were: lets a test see which launch configuration a host path chose (emu_launch_log below)
+static std::vector<std::pair<unsigned, size_t>> g_launch_log;
+static int										g_launch_count = 0;
+
 void launch(dim3 grid, unsigned block_threads, size_t dyn_smem_bytes, const std::function<void()> &fn)
 {
+	if (g_launch_log.size() < 4096) g_launch_log.emplace_back(block_threads, dyn_smem_bytes);
+	g_launch_count++;
 	g_grid_dim = grid;
 	g_block_dim = dim3(block_threads);
 	{
@@ -189,3 +198,18 @@ void launch(dim3 grid, unsigned block_threads, size_t dyn_smem_bytes, const std:
 }  // namespace emu
 
 extern "C" int emu_tma_unwaited() { return emu::g_tma_unwaited; }
+
+// Copies up to `cap` entries of the launch log (oldest first), clears it and returns how many launches there were since
+// it was last read.
+extern "C" int emu_launch_log(unsigned *threads, size_t *smem, int cap)
+{
+	const int n = emu::g_launch_count;
+	for (int i = 0; i < (int) emu::g_launch_log.size() && i < cap; i++)
+	{
+		threads[i] = emu::g_launch_log[i].first;
+		smem[i] = emu::g_launch_log[i].second;
+	}
+	emu::g_launch_log.clear();
+	emu::g_launch_count = 0;
+	return n;
+}

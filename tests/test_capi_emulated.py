@@ -579,3 +579,31 @@ def test_new_entry_points_argument_checks(pg):
     assert ol.tobytes() == want["labels"].tobytes()
     lib.pgemb_exchange_destroy(ex)
     idx.close()
+
+
+@pytest.fixture(scope="module")
+def DP():
+    import test_gpu_distance_paths as dp     # GPU tests of every distance path at the kernels' loop boundaries: bodies reused below
+    return dp
+
+
+@pytest.mark.parametrize("metric", ["l2", "cosine", "manhattan"])
+def test_distance_paths_entry_points(pg, DP, oracle_mod, metric):
+    """The discrimination guard on the emulated leg's dims, then pgemb_dist_batch / pgemb_dist_gather on them."""
+    DP.check_discrimination(oracle_mod, metric, DP.EMU_DIMS)
+    DP.check_dist_entry_points(pg, oracle_mod, metric, DP.EMU_DIMS)
+
+
+@pytest.mark.parametrize("metric", ["l2", "cosine", "manhattan"])
+def test_distance_paths_traversal(pg, DP, oracle_mod, metric, monkeypatch):
+    DP.check_traversal(pg, oracle_mod, metric, DP.EMU_DIMS, monkeypatch, latency_queries=2)
+
+
+@pytest.mark.parametrize("metric", ["l2", "cosine", "manhattan"])
+def test_distance_paths_scan(pg, DP, oracle_mod, metric, monkeypatch):
+    DP.check_scan(pg, oracle_mod, metric, DP.EMU_DIMS, monkeypatch)
+
+
+@pytest.mark.parametrize("metric", ["l2", "cosine", "manhattan"])
+def test_distance_paths_insert(pg, DP, oracle_mod, metric, monkeypatch):
+    DP.check_insert(pg, oracle_mod, metric, DP.EMU_INSERT_DIMS, monkeypatch, n=80)
