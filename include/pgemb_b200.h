@@ -206,6 +206,15 @@ void pgemb_scan_counters(uint64_t out[6]);
  * synchronised with on entry, the scan has finished when the call returns.  Same results, byte for byte. */
 pgemb_status pgemb_scan_topk_device(pgemb_index *idx, size_t nq, const coord_t *d_queries, size_t k, label_t *d_labels_out,
                                     dist_t *d_dists_out, int32_t *d_n_out, void *stream);
+/* The same two scans under any of the three operators, whatever the index's own metric is: `ORDER BY val <op> q LIMIT k`
+ * where <op> is not the opclass's (a relation indexed with ann_l2_ops queried with <=> or <~>).  Same contract, same paths
+ * (the tensor-core filter for L2 and cosine, the exact tiled kernel for manhattan) and the same counters; the distances are
+ * hnsw_dist_func(metric, ...)'s bits.  pgemb_scan_topk / pgemb_scan_topk_device are these calls with metric =
+ * idx->meta.dist_func.  A metric outside DIST_L2 .. DIST_MANHATTAN fails with PGEMB_ERR_ARG. */
+pgemb_status pgemb_scan_topk_op(pgemb_index *idx, dist_func_t metric, size_t nq, const coord_t *queries, size_t k, label_t *labels_out,
+                                dist_t *dists_out, int32_t *n_out);
+pgemb_status pgemb_scan_topk_op_device(pgemb_index *idx, dist_func_t metric, size_t nq, const coord_t *d_queries, size_t k,
+                                       label_t *d_labels_out, dist_t *d_dists_out, int32_t *d_n_out, void *stream);
 /* Test entry: the raw tensor-core products S[q][j] = q . row(r0 + j) (TF32 operands, fp32 accumulate) of the K6 kernel,
  * out[nq * nr], host pointers -- lets a test check descriptors / swizzle / accumulator layout against a float64 product. */
 pgemb_status pgemb_debug_umma_product(pgemb_index *idx, size_t nq, const coord_t *queries, size_t r0, size_t nr, float *out);

@@ -83,6 +83,12 @@ int pgemb_client_stats(uint64_t *n_batches, uint64_t *n_searches, uint64_t *max_
  * process's replica and honours the interrupt check and the dead-sidecar bound.  The scans that backends have pending at
  * the same time for the same (relation, k) are served by one pgemb_scan_topk call: one pass over the table for all of them. */
 int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, label_t *labels_out, dist_t *dists_out, size_t *n_out);
+/* The same scan under any of the three operators, whatever the relation's opclass is (pgemb_scan_topk_op): a relation indexed
+ * with ann_l2_ops and queried with <=> or <~>.  pgemb_client_scan_topk is this call with the mirror's own metric.  The pending
+ * scans of a relation are served by one call per (metric, k); a metric outside DIST_L2 .. DIST_MANHATTAN fails with
+ * PGEMB_ERR_ARG before anything is sent. */
+int pgemb_client_scan_topk_op(PgembClientIndex *h, dist_func_t metric, const coord_t *query, size_t k, label_t *labels_out, dist_t *dists_out,
+                              size_t *n_out);
 /* Sidecar scan counters, summed over replicas (largest batch: the maximum): pgemb_scan_topk calls, scans served, largest
  * batch.  Scans are not counted by pgemb_client_stats. */
 int pgemb_client_scan_stats(uint64_t *n_calls, uint64_t *n_scans, uint64_t *max_batch);

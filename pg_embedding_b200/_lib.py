@@ -39,7 +39,7 @@ ABI_SYMBOLS = [
     "pgemb_index_set_links", "pgemb_index_get_labels", "pgemb_index_set_labels",
     "pgemb_index_truncate", "pgemb_index_reserve", "pgemb_search_batch", "pgemb_search_batch_device",
     "pgemb_index_poll_error", "pgemb_last_kernel_ms", "pgemb_launch_count", "pgemb_dist_batch", "pgemb_dist_gather", "pgemb_scan_topk",
-    "pgemb_scan_counters", "pgemb_scan_topk_device", "pgemb_sharded_scan_device", "pgemb_debug_umma_product",
+    "pgemb_scan_counters", "pgemb_scan_topk_device", "pgemb_scan_topk_op", "pgemb_scan_topk_op_device", "pgemb_sharded_scan_device", "pgemb_debug_umma_product",
     "pgemb_index_scan_begin", "pgemb_index_scan_next", "pgemb_index_scan_next_batch", "pgemb_index_scan_ef", "pgemb_index_scan_searches",
     "pgemb_index_scan_end",
     "pgemb_bind_point", "pgemb_insert_batch", "pgemb_merge_topk_device", "pgemb_packed_topk_bytes", "pgemb_merge_topk_packed_device",
@@ -104,6 +104,7 @@ def _bind(lib: C.CDLL) -> C.CDLL:
     lib.pgemb_dist_batch.argtypes = [C.c_int, sz, sz, f32p, C.c_int, f32p, f32p]
     lib.pgemb_dist_gather.argtypes = [vp, sz, f32p, sz, u32p, f32p]
     lib.pgemb_scan_topk.argtypes = [vp, sz, f32p, sz, u64p, f32p, i32p]
+    lib.pgemb_scan_topk_op.argtypes = [vp, C.c_int, sz, f32p, sz, u64p, f32p, i32p]
     lib.pgemb_scan_counters.argtypes = [u64p]
     lib.pgemb_scan_counters.restype = None
     lib.pgemb_debug_umma_product.argtypes = [vp, sz, f32p, sz, sz, f32p]
@@ -133,6 +134,7 @@ def _bind(lib: C.CDLL) -> C.CDLL:
     lib.pgemb_sharded_search_device.argtypes = [vp, vp, sz, vp, sz, vp]
     lib.pgemb_sharded_scan_device.argtypes = [vp, vp, sz, vp, sz, vp]
     lib.pgemb_scan_topk_device.argtypes = [vp, sz, vp, sz, vp, vp, vp, vp]
+    lib.pgemb_scan_topk_op_device.argtypes = [vp, C.c_int, sz, vp, sz, vp, vp, vp, vp]
     lib.pgemb_sharded_merge_device.argtypes = [vp, sz, vp, vp, vp, vp]
     lib.pgemb_exchange_last_merge_ms.argtypes = [vp]
     lib.pgemb_exchange_last_merge_ms.restype = C.c_float

@@ -1257,6 +1257,7 @@ static pgemb_status launch_scan_filter(pgemb_index *idx, int metric, const float
 // so that a caller can switch them between calls.
 struct ScanPlan
 {
+	int	   metric;		  // the query's operator (DIST_*): any of the three, whatever the index's own metric is
 	bool   tc;			  // tensor-core filter + exact re-scoring; else the exact kernels alone
 	bool   tiled;		  // exact pass: scan_tile_kernel (same bits as scan_dist_kernel, rows read once per query tile)
 	int	   l2reset;		  // filter pass: what to give back of a traversal's L2 persistence window (scan_filter_pass)
@@ -1266,13 +1267,14 @@ struct ScanPlan
 	size_t growth, cmax;  // filter pass: chunk growth factor, largest chunk
 };
 
-static ScanPlan plan_scan(const pgemb_index *idx, size_t nq, size_t k, bool allow_tc)
+static ScanPlan plan_scan(const pgemb_index *idx, int metric, size_t nq, size_t k, bool allow_tc)
 {
 	ScanPlan p;
 	// PGEMB_SCAN_TC: 0 = exact kernels only, 1 (default) = tensor-core filter for L2 / cosine when the table has at least
 	// PGEMB_SCAN_TC_MIN_ROWS (default 4096) rows, 2 = always (tests).
 	const int mode = env_int("PGEMB_SCAN_TC", 1);
-	p.tc = allow_tc && idx->meta.dist_func != DIST_MANHATTAN && mode > 0 && (mode >= 2 || idx->n >= (size_t) env_int("PGEMB_SCAN_TC_MIN_ROWS", 4096));
+	p.metric = metric;
+	p.tc = allow_tc && metric != DIST_MANHATTAN && mode > 0 && (mode >= 2 || idx->n >= (size_t) env_int("PGEMB_SCAN_TC_MIN_ROWS", 4096));
 	p.tiled = env_int("PGEMB_SCAN_TILED", 1) != 0;
 	// PGEMB_SCAN_L2RESET: 0 = leave as is, 1 = reset lines + window, 2 (default) = also drop the set-aside limit until the next
 	// traversal configures it again
@@ -1335,7 +1337,7 @@ static pgemb_status scan_filter_pass(pgemb_index *idx, const ScanPlan &p, const 
 	}
 	pgemb_status st = ensure_row_norms(idx, s);
 	if (st) return st;
-	const int	 metric = (int) idx->meta.dist_func;
+	const int	 metric = p.metric;
 	const size_t N = idx->n, dim = idx->meta.dim, rf = idx->row_f;
 	CU_TRY(cudaMemsetAsync(b.cnt, 0, 16, s));
 	st = with_tc_metric(metric, [&](auto m) -> pgemb_status {
@@ -1372,9 +1374,15 @@ static pgemb_status scan_filter_pass(pgemb_index *idx, const ScanPlan &p, const 
 // the exact kernels: per chunk of rows, every (query, row) distance, then its fold into the running top-k
 static pgemb_status scan_exact_pass(pgemb_index *idx, const ScanPlan &p, const ScanBuffers &b, size_t nq, size_t k, cudaStream_t s)
 {
-	const int	   metric = (int) idx->meta.dist_func;
+	const int	   metric = p.metric;
 	const size_t   N = idx->n, dim = idx->meta.dim, rf = idx->row_f;
 	const uint32_t lanes = (metric == DIST_L2) ? 8 : 4;
+	if (metric == DIST_COSINE)
+	{
+		// the cosine epilogue divides by the row norms: a mirror of another metric computes them on its first cosine scan
+		const pgemb_status st = ensure_row_norms(idx, s);
+		if (st) return st;
+	}
 	g_scan_exact++;
 	for (size_t r0 = 0; r0 < N; r0 += p.chunk)
 	{
@@ -1427,13 +1435,13 @@ static pgemb_status scan_hand_off(const ScanBuffers &b, size_t nq, size_t k, lab
 
 // One group of queries: stage them, run one pass over the table, hand the results over.  *tc_violation: the tensor-core
 // filter saw a product outside its assumed error bound.
-static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
+static pgemb_status scan_topk_impl(pgemb_index *idx, int metric, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
 								   int32_t *n_out, bool allow_tc, bool *tc_violation, bool device_io)
 {
 	*tc_violation = false;
 	pgemb_status st = set_device(idx);
 	if (st) return st;
-	const ScanPlan p = plan_scan(idx, nq, k, allow_tc);
+	const ScanPlan p = plan_scan(idx, metric, nq, k, allow_tc);
 	cudaStream_t   s = idx->stream;
 	const size_t   qb = nq * idx->row_f * 4, db = p.tc ? 0 : nq * p.chunk * 4, kd = nq * k * 4, kl = nq * k * 8, nb = nq * 4;
 	const size_t   cb = p.tc ? nq * p.cap * 4 : 0;
@@ -1446,7 +1454,7 @@ static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *q
 	st = stage_queries(idx, b.q, queries, nq, device_io ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s);
 	if (st) return st;
 	CU_TRY(cudaMemsetAsync(b.tn, 0, nb, s));
-	if (p.tc || (p.tiled && idx->meta.dist_func == DIST_COSINE))
+	if (p.tc || (p.tiled && metric == DIST_COSINE))
 	{
 		PGEMB_LAUNCH(norms_kernel, (uint32_t) ((nq * 4 + 127) / 128), 128, 0, s, b.q, idx->row_f, (uint32_t) idx->meta.dim, 0u, (uint32_t) nq, b.qn);
 		g_launches++;
@@ -1466,10 +1474,11 @@ static pgemb_status scan_topk_impl(pgemb_index *idx, size_t nq, const coord_t *q
 	return PGEMB_OK;
 }
 
-static pgemb_status scan_topk_groups(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out, int32_t *n_out,
-									 bool device_io)
+static pgemb_status scan_topk_groups(pgemb_index *idx, int metric, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
+									 int32_t *n_out, bool device_io)
 {
 	if (!idx || ((!queries || !labels_out || !n_out) && nq)) return fail(PGEMB_ERR_ARG, "null argument");
+	if (metric < 0 || metric > 2) return fail(PGEMB_ERR_ARG, "unknown distance function");
 	if (nq == 0) return PGEMB_OK;
 	if (k < 1 || k > 4096) return fail(PGEMB_ERR_ARG, "k out of range (1..4096)");
 	if (nq > (1u << 20)) return fail(PGEMB_ERR_ARG, "too many queries in one scan batch");
@@ -1479,14 +1488,14 @@ static pgemb_status scan_topk_groups(pgemb_index *idx, size_t nq, const coord_t 
 	{
 		const size_t gq = nq - q0 < group ? nq - q0 : group;
 		bool		 viol = false;
-		pgemb_status st = scan_topk_impl(idx, gq, queries + q0 * idx->meta.dim, k, labels_out + q0 * k, dists_out ? dists_out + q0 * k : nullptr, n_out + q0,
+		pgemb_status st = scan_topk_impl(idx, metric, gq, queries + q0 * idx->meta.dim, k, labels_out + q0 * k, dists_out ? dists_out + q0 * k : nullptr, n_out + q0,
 										 true, &viol, device_io);
 		if (st == PGEMB_OK && viol)
 		{
 			// the tensor-core filter saw a product outside its assumed error bound: its result is not trusted
 			g_scan_fallbacks++;
 			fprintf(stderr, "pgemb_scan_topk: tensor-core error bound exceeded, repeating the scan on the exact kernels\n");
-			st = scan_topk_impl(idx, gq, queries + q0 * idx->meta.dim, k, labels_out + q0 * k, dists_out ? dists_out + q0 * k : nullptr, n_out + q0, false, &viol,
+			st = scan_topk_impl(idx, metric, gq, queries + q0 * idx->meta.dim, k, labels_out + q0 * k, dists_out ? dists_out + q0 * k : nullptr, n_out + q0, false, &viol,
 								device_io);
 		}
 		if (st) return st;
@@ -1494,16 +1503,23 @@ static pgemb_status scan_topk_groups(pgemb_index *idx, size_t nq, const coord_t 
 	return PGEMB_OK;
 }
 
+extern "C" pgemb_status pgemb_scan_topk_op(pgemb_index *idx, dist_func_t metric, size_t nq, const coord_t *queries, size_t k, label_t *labels_out,
+										   dist_t *dists_out, int32_t *n_out)
+{
+	return scan_topk_groups(idx, (int) metric, nq, queries, k, labels_out, dists_out, n_out, false);
+}
+
 extern "C" pgemb_status pgemb_scan_topk(pgemb_index *idx, size_t nq, const coord_t *queries, size_t k, label_t *labels_out, dist_t *dists_out,
 										int32_t *n_out)
 {
-	return scan_topk_groups(idx, nq, queries, k, labels_out, dists_out, n_out, false);
+	if (!idx) return fail(PGEMB_ERR_ARG, "null argument");
+	return pgemb_scan_topk_op(idx, idx->meta.dist_func, nq, queries, k, labels_out, dists_out, n_out);
 }
 
 // The same scan with DEVICE pointers in and out (the caller's stream is only synchronised with: the scan runs on the index's own
 // stream and has finished when the call returns).  For callers whose queries and results live in HBM already: the sharded scan.
-extern "C" pgemb_status pgemb_scan_topk_device(pgemb_index *idx, size_t nq, const coord_t *d_queries, size_t k, label_t *d_labels_out, dist_t *d_dists_out,
-											   int32_t *d_n_out, void *stream)
+extern "C" pgemb_status pgemb_scan_topk_op_device(pgemb_index *idx, dist_func_t metric, size_t nq, const coord_t *d_queries, size_t k, label_t *d_labels_out,
+												  dist_t *d_dists_out, int32_t *d_n_out, void *stream)
 {
 	if (idx && stream)
 	{
@@ -1511,7 +1527,14 @@ extern "C" pgemb_status pgemb_scan_topk_device(pgemb_index *idx, size_t nq, cons
 		if (st) return st;
 		CU_TRY(cudaStreamSynchronize((cudaStream_t) stream));  // the queries may have been produced on it
 	}
-	return scan_topk_groups(idx, nq, d_queries, k, d_labels_out, d_dists_out, d_n_out, true);
+	return scan_topk_groups(idx, (int) metric, nq, d_queries, k, d_labels_out, d_dists_out, d_n_out, true);
+}
+
+extern "C" pgemb_status pgemb_scan_topk_device(pgemb_index *idx, size_t nq, const coord_t *d_queries, size_t k, label_t *d_labels_out, dist_t *d_dists_out,
+											   int32_t *d_n_out, void *stream)
+{
+	if (!idx) return fail(PGEMB_ERR_ARG, "null argument");
+	return pgemb_scan_topk_op_device(idx, idx->meta.dist_func, nq, d_queries, k, d_labels_out, d_dists_out, d_n_out, stream);
 }
 
 // Debug / test entry: the raw tensor-core products S[q][j] = q . row(r0 + j) of the K6 kernel (TF32 operands, fp32

@@ -518,11 +518,13 @@ int pgemb_client_dist_stats(uint64_t *n_calls, uint64_t *n_dists, uint64_t *max_
 }
 
 /* ---- the index-less scan (embedding.c:1022-1062 per row + the executor's sort; knn.out:63-91) ------------------------- */
-int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, label_t *labels_out, dist_t *dists_out, size_t *n_out)
+/* metric_code: ipc.h's PGEMB_OP_SCAN a1 (0 = the mirror's metric, else 1 + dist_func_t); fn: the caller's name for messages */
+static int scan_topk(const char *fn, PgembClientIndex *h, uint64_t metric_code, const coord_t *query, size_t k, label_t *labels_out, dist_t *dists_out,
+					 size_t *n_out)
 {
 	if (!h || !query || !labels_out || !n_out)
 	{
-		set_err("pgemb_client_scan_topk: null argument");
+		set_err("%s: null argument", fn);
 		return PGEMB_ERR_ARG;
 	}
 	int rc = ensure_connected();
@@ -531,17 +533,18 @@ int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, 
 	const size_t kmax = c->hdr->max_ef < 4096 ? c->hdr->max_ef : 4096;
 	if (k < 1 || k > kmax)
 	{
-		set_err("pgemb_client_scan_topk: k = %zu outside 1 .. %zu (min(4096, the sidecar's --max-ef))", k, kmax);
+		set_err("%s: k = %zu outside 1 .. %zu (min(4096, the sidecar's --max-ef))", fn, k, kmax);
 		return PGEMB_ERR_ARG;
 	}
 	if (h->meta.dim < 1 || h->meta.dim > c->hdr->max_dim)
 	{
-		set_err("pgemb_client_scan_topk: dims outside the sidecar's limits");
+		set_err("%s: dims outside the sidecar's limits", fn);
 		return PGEMB_ERR_ARG;
 	}
 	PgembIpcSlot *s = claim_slot(c, PGEMB_OP_SCAN, h->rel_key);
 	if (!s) return PGEMB_ERR_STATE;
 	s->a0 = k;
+	s->a1 = metric_code;
 	memcpy(slot_vec(s), query, h->meta.dim * sizeof(coord_t));
 	rc = submit_wait(c, s);
 	if (rc == PGEMB_OK)
@@ -555,11 +558,27 @@ int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, 
 		}
 		else
 		{
-			set_err("pgemb_client_scan_topk: the sidecar returned %d results for k = %zu", (int) s->n_out, k);
+			set_err("%s: the sidecar returned %d results for k = %zu", fn, (int) s->n_out, k);
 			rc = PGEMB_ERR_STATE;
 		}
 	}
 	return end_request(s, rc);
+}
+
+int pgemb_client_scan_topk(PgembClientIndex *h, const coord_t *query, size_t k, label_t *labels_out, dist_t *dists_out, size_t *n_out)
+{
+	return scan_topk("pgemb_client_scan_topk", h, 0, query, k, labels_out, dists_out, n_out);
+}
+
+int pgemb_client_scan_topk_op(PgembClientIndex *h, dist_func_t metric, const coord_t *query, size_t k, label_t *labels_out, dist_t *dists_out,
+							  size_t *n_out)
+{
+	if ((int) metric < 0 || (int) metric > 2)
+	{
+		set_err("pgemb_client_scan_topk_op: unknown distance function %d", (int) metric);
+		return PGEMB_ERR_ARG;
+	}
+	return scan_topk("pgemb_client_scan_topk_op", h, 1 + (uint64_t) metric, query, k, labels_out, dists_out, n_out);
 }
 
 int pgemb_client_shutdown_server(void) { return simple_request(1, NULL, PGEMB_OP_SHUTDOWN, 0, 0, 0, 0, NULL, NULL, NULL); }

@@ -7,8 +7,8 @@
  * so the device index has to live in one GPU-owning process and be keyed by relation.  The reference calls
  * hnsw_search one query at a time (embedding.c:317,335); many backends doing so concurrently is exactly the batch the
  * traversal kernel wants, so the sidecar gathers the requests that are pending at the same time into ONE
- * pgemb_search_batch launch.  Index-less scans (PGEMB_OP_SCAN) are gathered the same way, per (relation, k), into one
- * pgemb_scan_topk call, and one-pair distances (PGEMB_OP_DIST), per (metric, dim), into one pgemb_dist_batch call.
+ * pgemb_search_batch launch.  Index-less scans (PGEMB_OP_SCAN) are gathered the same way, per (relation, metric, k), into
+ * one pgemb_scan_topk_op call, and one-pair distances (PGEMB_OP_DIST), per (metric, dim), into one pgemb_dist_batch call.
  *
  * One POSIX shared-memory segment:
  *     IpcHeader | IpcSlot[n_slots] (each followed by its payload) | bulk area
@@ -28,7 +28,7 @@
 #include <stddef.h>
 
 #define PGEMB_IPC_MAGIC 0x424d4750u /* "PGMB" */
-#define PGEMB_IPC_VERSION 3u
+#define PGEMB_IPC_VERSION 4u /* 4: PGEMB_OP_SCAN carries the query's metric in a1 */
 
 enum
 {
@@ -55,7 +55,8 @@ enum
 	PGEMB_OP_BUILD = 12,		  /* a0 = first, a1 = n, a2 = batch_max, a3 = 1: exact (bit-identical to row-by-row), 0: bulk */
 	PGEMB_OP_DIST = 13,			  /* a0 = dim, a1 = metric, payload: a[dim] b[dim] -> a2 = fp32 bits (hnsw_dist_func) */
 	PGEMB_OP_SHUTDOWN = 14,
-	PGEMB_OP_SCAN = 15			  /* a0 = k, payload: query[dim] -> n_out, labels[n_out], dists[n_out] (pgemb_scan_topk for one query) */
+	PGEMB_OP_SCAN = 15			  /* a0 = k, a1 = 0 (the mirror's metric) or 1 + dist_func_t, payload: query[dim] -> n_out, labels[n_out],
+									   dists[n_out] (pgemb_scan_topk_op for one query) */
 };
 
 typedef struct

@@ -5,7 +5,7 @@
 // hnsw_search one query per call, one call per backend at a time (embedding.c:317,335) -- are gathered per
 // (relation, efSearch) into ONE pgemb_search_batch launch: a single query cannot fill an H100, the concurrent queries
 // of many backends can (DESIGN.md section 6).  Index-less scans (`ORDER BY val <op> q LIMIT k` without the index) are
-// gathered the same way per (relation, k) into ONE pgemb_scan_topk call: every scan reads the whole table, so sharing
+// gathered the same way per (relation, metric, k) into ONE pgemb_scan_topk_op call: every scan reads the whole table, so sharing
 // that read pays even more there (DESIGN.md section 12).  The SQL distance operators' hnsw_dist_func calls (one pair each,
 // embedding.c:1022-1062) are gathered per (metric, dim) into ONE pgemb_dist_batch call.  Everything else (mirror maintenance,
 // hnsw_bind_point, link write-back) is run one request at a time, which is also the reference's rule for writers
@@ -57,7 +57,7 @@ struct Api
 	pgemb_status (*truncate)(pgemb_index *);
 	pgemb_status (*reserve)(pgemb_index *, size_t);
 	pgemb_status (*search_batch)(pgemb_index *, size_t, const coord_t *, size_t, label_t *, dist_t *, idx_t *, int32_t *, uint32_t *);
-	pgemb_status (*scan_topk)(pgemb_index *, size_t, const coord_t *, size_t, label_t *, dist_t *, int32_t *);
+	pgemb_status (*scan_topk_op)(pgemb_index *, dist_func_t, size_t, const coord_t *, size_t, label_t *, dist_t *, int32_t *);
 	pgemb_status (*dist_batch)(dist_func_t, size_t, size_t, const coord_t *, int, const coord_t *, dist_t *);
 	bool (*bind_point)(HnswMetadata *, const coord_t *, idx_t);	 // the reference-shaped hnsw_bind_point
 	pgemb_status (*build_bulk)(pgemb_index *, size_t, size_t, size_t, double *);
@@ -85,7 +85,7 @@ bool load_api(const char *path, Api &a)
 		   sym(h, "pgemb_index_capacity", a.index_capacity) && sym(h, "pgemb_index_append_records", a.append_records) &&
 		   sym(h, "pgemb_index_export_records", a.export_records) && sym(h, "pgemb_index_get_links", a.get_links) &&
 		   sym(h, "pgemb_index_set_labels", a.set_labels) && sym(h, "pgemb_index_truncate", a.truncate) && sym(h, "pgemb_index_reserve", a.reserve) && sym(h, "pgemb_search_batch", a.search_batch) &&
-		   sym(h, "pgemb_scan_topk", a.scan_topk) && sym(h, "pgemb_dist_batch", a.dist_batch) && sym(h, "hnsw_bind_point", a.bind_point) && sym(h, "pgemb_build_bulk", a.build_bulk) && sym(h, "pgemb_build_exact", a.build_exact) &&
+		   sym(h, "pgemb_scan_topk_op", a.scan_topk_op) && sym(h, "pgemb_dist_batch", a.dist_batch) && sym(h, "hnsw_bind_point", a.bind_point) && sym(h, "pgemb_build_bulk", a.build_bulk) && sym(h, "pgemb_build_exact", a.build_exact) &&
 		   sym(h, "hnsw_init_dist_func", a.init_dist_func);
 }
 
@@ -105,8 +105,9 @@ double now_s()
 volatile sig_atomic_t g_stop = 0;
 void				  on_signal(int) { g_stop = 1; }
 
-// A batched group: (PGEMB_OP_SEARCH, relation, ef), (PGEMB_OP_SCAN, relation, k) or (PGEMB_OP_DIST, metric, dim)
-using GroupKey = std::tuple<uint32_t, uint64_t, uint64_t>;
+// A batched group: (PGEMB_OP_SEARCH, relation, ef, 0), (PGEMB_OP_SCAN, relation, k, metric code) or (PGEMB_OP_DIST, metric, dim, 0).
+// A scan's metric code is ipc.h's a1: 1 + dist_func_t, or 0 = the mirror's metric (resolved by collect() when the mirror exists).
+using GroupKey = std::tuple<uint32_t, uint64_t, uint64_t, uint64_t>;
 
 struct Server
 {
@@ -335,12 +336,13 @@ struct Server
 	}
 
 	// ---- batched requests: all pending requests of one group -> one library call per max_batch --------------------
-	// Searches launch pgemb_search_batch, scans pgemb_scan_topk and distances pgemb_dist_batch.  Scans are grouped by k, not
-	// folded into the largest k of the relation: a query's re-scoring work grows with k (DESIGN.md section 6).  Every
-	// distance pair is independent and gets the bits of a one-pair call: the same dist_pairs_kernel evaluates each pair alone.
+	// Searches launch pgemb_search_batch, scans pgemb_scan_topk_op and distances pgemb_dist_batch.  Scans are grouped by metric
+	// (one pass over the table serves one operator) and by k, not folded into the largest k of the relation: a query's
+	// re-scoring work grows with k (DESIGN.md section 6).  Every distance pair is independent and gets the bits of a one-pair
+	// call: the same dist_pairs_kernel evaluates each pair alone.
 	void run_group(const GroupKey &key, const std::vector<PgembIpcSlot *> &group)
 	{
-		const auto [op, g, k] = key;  // g: relation key (search, scan) or metric (distance); k: ef, k or dim
+		const auto [op, g, k, mc] = key;  // g: relation key (search, scan) or metric (distance); k: ef, k or dim; mc: scan metric code
 		PgembHostIndex *m = nullptr;
 		const char	   *bad = nullptr;
 		if (op == PGEMB_OP_DIST)
@@ -354,6 +356,8 @@ struct Server
 			bad = "efSearch outside the sidecar's --max-ef";
 		else if (op == PGEMB_OP_SCAN && (k < 1 || k > std::min<size_t>(4096, hdr->max_ef)))
 			bad = "scan: k outside 1 .. min(4096, the sidecar's --max-ef)";
+		else if (op == PGEMB_OP_SCAN && mc > 3)
+			bad = "scan: unknown distance function";
 		else
 			m = &it->second;
 		if (bad)
@@ -396,7 +400,8 @@ struct Server
 				lbuf.resize(nq * k);
 				dbuf.resize(nq * k);
 				nbuf.assign(nq, 0);
-				r = api.scan_topk(m->dev, nq, qbuf.data(), k, lbuf.data(), dbuf.data(), nbuf.data());
+				const dist_func_t metric = mc ? (dist_func_t) (mc - 1) : m->meta.dist_func;
+				r = api.scan_topk_op(m->dev, metric, nq, qbuf.data(), k, lbuf.data(), dbuf.data(), nbuf.data());
 				count(hdr->n_scan_calls, hdr->n_scans, hdr->max_scan_batch);
 			}
 			else
@@ -443,20 +448,26 @@ struct Server
 				found++;
 				if (s->op == PGEMB_OP_SEARCH)
 				{
-					batched[{s->op, s->index_key, s->ef}].push_back(s);
+					batched[{s->op, s->index_key, s->ef, 0}].push_back(s);
 					nsearch++;
 				}
 				else if (s->op == PGEMB_OP_SCAN)
-					batched[{s->op, s->index_key, s->a0}].push_back(s);  // not part of the searches' linger bookkeeping (nsearch / target / carry)
+				{
+					// not part of the searches' linger bookkeeping (nsearch / target / carry).  A scan that asks for the mirror's
+					// metric joins the group of the scans that name that metric.
+					uint64_t mc = s->a1;
+					if (auto it = mirrors.find(s->index_key); mc == 0 && it != mirrors.end()) mc = 1 + (uint64_t) it->second.meta.dist_func;
+					batched[{s->op, s->index_key, s->a0, mc}].push_back(s);
+				}
 				else if (s->op == PGEMB_OP_DIST)
-					batched[{s->op, s->a1, s->a0}].push_back(s);	 // touches no mirror, so no place in the write/search order; never lingers
+					batched[{s->op, s->a1, s->a0, 0}].push_back(s);	 // touches no mirror, so no place in the write/search order; never lingers
 				else
 					control.push_back(s);
 			}
 		};
 		// serve every collected group of one kind, in key order
 		auto run_groups = [&](uint32_t op) {
-			const auto first = batched.lower_bound(GroupKey{op, 0, 0}), last = batched.lower_bound(GroupKey{op + 1, 0, 0});
+			const auto first = batched.lower_bound(GroupKey{op, 0, 0, 0}), last = batched.lower_bound(GroupKey{op + 1, 0, 0, 0});
 			for (auto it = first; it != last; ++it) run_group(it->first, it->second);
 			batched.erase(first, last);
 		};

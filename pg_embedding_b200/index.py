@@ -295,15 +295,20 @@ class HnswIndex:
             self.last_scan = {"ef": int(self.lib.pgemb_index_scan_ef(sc)), "searches": int(self.lib.pgemb_index_scan_searches(sc))}
             self.lib.pgemb_index_scan_end(sc)
 
-    def scan_topk(self, queries, k: int):
-        """Exact brute-force k-NN (the seq-scan answer, knn.out:63-91), batched. Returns dict(labels, dists, n)."""
+    def scan_topk(self, queries, k: int, metric=None):
+        """Exact brute-force k-NN (the seq-scan answer, knn.out:63-91), batched. Returns dict(labels, dists, n).
+        `metric` (name or DIST_*): the query's operator, any of the three; None = the index's own."""
         q = _f32(queries)
         self._check_dims(q)
         nq = q.shape[0]
         labels = np.empty((nq, k), dtype=np.uint64)
         dists = np.empty((nq, k), dtype=np.float32)
         n = np.zeros(nq, dtype=np.int32)
-        check(self.lib.pgemb_scan_topk(self.dev, nq, _p(q, C.c_float), int(k), _p(labels, C.c_uint64), _p(dists, C.c_float), _p(n, C.c_int32)))
+        out = (_p(q, C.c_float), int(k), _p(labels, C.c_uint64), _p(dists, C.c_float), _p(n, C.c_int32))
+        if metric is None:
+            check(self.lib.pgemb_scan_topk(self.dev, nq, *out))
+        else:
+            check(self.lib.pgemb_scan_topk_op(self.dev, _metric(metric), nq, *out))
         return {"labels": labels, "dists": dists, "n": n}
 
     def dist_gather(self, queries, ids) -> np.ndarray:

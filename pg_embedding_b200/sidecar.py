@@ -61,6 +61,7 @@ def client() -> C.CDLL:
     lib.pgemb_client_scan_stats.argtypes = [C.POINTER(C.c_uint64)] * 3
     lib.pgemb_client_dist_stats.argtypes = [C.POINTER(C.c_uint64)] * 3
     lib.pgemb_client_scan_topk.argtypes = [hp, C.POINTER(C.c_float), sz, C.POINTER(C.c_uint64), C.POINTER(C.c_float), C.POINTER(sz)]
+    lib.pgemb_client_scan_topk_op.argtypes = [hp, C.c_int, C.POINTER(C.c_float), sz, C.POINTER(C.c_uint64), C.POINTER(C.c_float), C.POINTER(sz)]
     lib.pgemb_client_set_interrupt_check.argtypes = [C.c_void_p]
     lib.hnsw_search.argtypes = [C.POINTER(HnswMetadata), C.POINTER(C.c_float), C.POINTER(sz), C.POINTER(C.POINTER(C.c_uint64))]
     lib.hnsw_search.restype = C.c_bool
@@ -215,17 +216,22 @@ class RemoteIndex:
         finally:
             self.h.meta.efSearch = ef0      # the reference's HnswIndex is per scan (embedding.c:254)
 
-    def scan_topk(self, q: np.ndarray, k: int) -> dict:
+    def scan_topk(self, q: np.ndarray, k: int, metric=None) -> dict:
         """`ORDER BY val <op> q LIMIT k` without the index (knn.out:63-91) for one query, through the sidecar's batched
-        pgemb_scan_topk.  Returns dict(labels[k], dists[k], n) -- one row of HnswIndex.scan_topk (unused tail: ~0 / inf)."""
+        pgemb_scan_topk.  Returns dict(labels[k], dists[k], n) -- one row of HnswIndex.scan_topk (unused tail: ~0 / inf).
+        `metric` (name or DIST_* number): the query's operator, any of the three; None = the relation's own."""
         q = np.ascontiguousarray(q, dtype=np.float32).ravel()
         if q.size != self.dims:
             raise ValueError(f"Wrong number of dimensions: {q.size} instead of {self.dims} expected")
         labels = np.full(max(int(k), 1), np.iinfo(np.uint64).max, np.uint64)
         dists = np.full(max(int(k), 1), np.inf, np.float32)
         n = C.c_size_t()
-        _check(client().pgemb_client_scan_topk(C.byref(self.h), q.ctypes.data_as(C.POINTER(C.c_float)), int(k),
-                                               labels.ctypes.data_as(C.POINTER(C.c_uint64)), dists.ctypes.data_as(C.POINTER(C.c_float)), C.byref(n)))
+        out = (q.ctypes.data_as(C.POINTER(C.c_float)), int(k), labels.ctypes.data_as(C.POINTER(C.c_uint64)),
+               dists.ctypes.data_as(C.POINTER(C.c_float)), C.byref(n))
+        if metric is None:
+            _check(client().pgemb_client_scan_topk(C.byref(self.h), *out))
+        else:
+            _check(client().pgemb_client_scan_topk_op(C.byref(self.h), METRICS[metric] if isinstance(metric, str) else int(metric), *out))
         return {"labels": labels, "dists": dists, "n": n.value}
 
     def bind_point(self, idx: int, efconstruction: int | None = None) -> None:
