@@ -47,6 +47,9 @@ struct BindWorkspace
 	uint64_t *d_pairs_sorted = nullptr;
 	void	 *d_cub = nullptr;
 	size_t	  cub_bytes = 0;
+	// select_global_kernel only (efConstruction beyond a CTA's shared memory): candidate keys and scan order, [points][ef]
+	uint64_t *d_sel_keys = nullptr;
+	uint32_t *d_sel_ord = nullptr;
 	// exact parallel build (speculative batches)
 	static constexpr uint32_t kExpCap = 1024;
 	uint32_t *d_exp = nullptr;		 // [points][kExpCap] expanded nodes of each speculative search
@@ -65,6 +68,8 @@ inline void bind_ws_free(BindWorkspace &w)
 	cudaFree(w.d_pairs);
 	cudaFree(w.d_pairs_sorted);
 	cudaFree(w.d_cub);
+	cudaFree(w.d_sel_keys);
+	cudaFree(w.d_sel_ord);
 	cudaFree(w.d_exp);
 	cudaFree(w.d_exp_n);
 	cudaFree(w.d_stamp);
@@ -301,6 +306,62 @@ __global__ void __launch_bounds__(kBindThreads) select_kernel(GraphView g, const
 	}
 }
 
+// The same select with the candidate keys and the scan order in the bind workspace (keys, ord: [n_new][ef]) and only the
+// kept keys in shared memory: for an efConstruction whose 12 x ef bytes exceed a CTA's shared memory.  Same heuristic, same
+// order, same arithmetic -- the same lists.  A copy of select_kernel's unstaged body: moving that body into a shared device function
+// changed the instructions nvcc emits for select_kernel, whose measured code stays as it is.
+template <int METRIC>
+__global__ void __launch_bounds__(kBindThreads) select_global_kernel(GraphView g, const uint32_t *__restrict__ new_ids,
+																	  const uint32_t *__restrict__ cand_ids, const float *__restrict__ cand_d,
+																	  const int32_t *__restrict__ cand_n, uint32_t ef,
+																	  uint64_t *__restrict__ pairs, uint64_t *__restrict__ keys,
+																	  uint32_t *__restrict__ ords)
+{
+	PGEMB_DYNAMIC_SMEM(sm, 16);
+	uint64_t	  *cand = keys + (size_t) blockIdx.x * ef;			// ef, in the workspace
+	uint64_t	  *kept = reinterpret_cast<uint64_t *>(sm);			// max(M,1)
+	uint32_t	  *ord = ords + (size_t) blockIdx.x * ef;			// ef, in the workspace
+	const uint32_t b = blockIdx.x;
+	const uint32_t cur = new_ids[b];
+	uint64_t	  *my_pairs = pairs + (size_t) b * (g.M ? g.M : 1);
+	for (uint32_t i = threadIdx.x; i < g.M; i += kBindThreads) my_pairs[i] = ~0ull;
+	if (cur == 0) return;  // "Do nothing for the first element", hnswalg.cpp:227-228
+	const uint32_t C = (uint32_t) max(0, cand_n[b]);
+	for (uint32_t i = threadIdx.x; i < C; i += kBindThreads)
+		cand[i] = make_key(cand_d[(size_t) b * ef + i], cand_ids[(size_t) b * ef + i]);
+	__syncthreads();
+	uint32_t		nsel;
+	const uint64_t *sel;
+	if (C < g.M)
+	{
+		nsel = C;  // hnswalg.cpp:119-120: fewer than NN candidates -> all of them
+		sel = cand;
+	}
+	else
+	{
+		nsel = heuristic_block<METRIC>(g, cand, C, g.M, ord, kept);
+		sel = kept;
+	}
+	__syncthreads();
+	uint32_t *L = g.links + (size_t) cur * g.link_stride;
+	// "Should be blank" (hnswalg.cpp:170-171, :176-177)
+	int bad = 0;
+	for (uint32_t i = threadIdx.x; i <= nsel && i <= g.maxM; i += kBindThreads) bad |= (L[i] != 0u);
+	if (__syncthreads_or(bad))
+	{
+		if (threadIdx.x == 0) *g.error_flag = 3;
+		return;
+	}
+	write_list_desc(L, sel, nsel);
+	// back-link work items, keyed (target, source) so that a sort serialises equal targets by source id
+	for (uint32_t i = threadIdx.x; i < nsel; i += kBindThreads)
+	{
+		const uint32_t s = key_id(sel[i]);
+		if (s == cur) *g.error_flag = 3;  // "Connection to the same element" (hnswalg.cpp:183-184)
+		my_pairs[i] = ((uint64_t) s << 32) | (uint64_t) cur;
+	}
+}
+
 // dynamic shared memory of select_kernel: candidate keys, kept keys, scan order (+ the staged rows)
 inline size_t select_smem_bytes(size_t ef, size_t M, size_t row_f, bool staged)
 {
@@ -308,6 +369,9 @@ inline size_t select_smem_bytes(size_t ef, size_t M, size_t row_f, bool staged)
 	if (!staged) return base;
 	return (base + 15) / 16 * 16 + 16 + ((M ? M : 1) + 2) * row_f * 4;
 }
+
+// dynamic shared memory of select_global_kernel: the kept keys
+inline size_t select_global_smem_bytes(size_t M) { return (M ? M : 1) * 8; }
 
 // ---- back-links: one CTA per run of equal targets in the sorted (target,source) array ----------------
 template <int METRIC>

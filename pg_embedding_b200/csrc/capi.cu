@@ -1841,6 +1841,25 @@ static pgemb_status launch_select(pgemb_index *idx, const uint32_t *d_new_ids, s
 	BindWorkspace  &w = idx->bind_ws;
 	const GraphView g = graph_view(idx);
 	const size_t	sel_smem = select_smem_bytes(ef, idx->meta.M, idx->row_f, staged);
+	if (sel_smem > kMaxCtaSmem)
+	{
+		// efConstruction beyond shared memory (12 x ef bytes): the candidate keys and the scan order go to the workspace
+		if (!w.d_sel_keys)
+		{
+			CU_TRY(cudaMalloc((void **) &w.d_sel_keys, w.cap_points * w.cap_ef * sizeof(uint64_t)));
+			CU_TRY(cudaMalloc((void **) &w.d_sel_ord, w.cap_points * w.cap_ef * sizeof(uint32_t)));
+		}
+		const size_t kept_smem = select_global_smem_bytes(idx->meta.M);
+		return with_metric((int) idx->meta.dist_func, [&](auto m) -> pgemb_status {
+			const auto fn = select_global_kernel<decltype(m)::value>;
+			if (kept_smem > 48 * 1024) CU_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kept_smem));
+			PGEMB_LAUNCH(fn, (uint32_t) count, kBindThreads, kept_smem, s, g, d_new_ids, w.d_cand_ids, w.d_cand_d, w.d_cand_n, (uint32_t) ef, w.d_pairs,
+						 w.d_sel_keys, w.d_sel_ord);
+			g_launches++;
+			CU_TRY(cudaGetLastError());
+			return PGEMB_OK;
+		});
+	}
 	return with_metric((int) idx->meta.dist_func, [&](auto m) -> pgemb_status {
 		const auto fn = staged ? select_kernel<decltype(m)::value, true> : select_kernel<decltype(m)::value, false>;
 		if (sel_smem > 48 * 1024) CU_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sel_smem));

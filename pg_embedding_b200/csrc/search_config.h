@@ -20,6 +20,7 @@ struct RingPool
 	float	 coop_qn;
 };
 constexpr uint32_t kMaxRings = 15;
+constexpr uint32_t kMaxCtaSmem = 232448u;  // dynamic shared memory a CTA may opt in to on the H100 (227 KB)
 
 struct SearchConfig
 {
@@ -65,7 +66,7 @@ inline int make_search_config(const SearchShape &sh, const SearchTuning &tu, boo
 	if (row_smem < row_bytes) row_smem += 128u;
 	const uint32_t maxM = sh.maxM;
 	const uint32_t hopcap = maxM > 1 ? maxM : 1;
-	const uint32_t max_cta = 232448u;  // 227 KB per CTA
+	const uint32_t max_cta = kMaxCtaSmem;
 	const uint32_t ef = sh.ef;
 	if (!sh.res_global && ef > (max_cta / 16u)) return 1;  // 2 x ef x 8 bytes alone exceed a CTA's shared memory
 	// lane-major transposed query: per lane-thread a run of floats padded so that the four runs start

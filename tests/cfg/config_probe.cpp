@@ -11,7 +11,7 @@ int main()
 	printf("metric,dim,maxM,ef,coop,tpr,rc,warps,rings,ring_bytes,priv_bytes,row_smem,qt_stride,smem,slots,off_pool,off_ring,off_priv,off_qt,off_qtail,off_res,off_hopkey,off_acckey,off_evict,off_hopid,off_pf,off_pfbar,pool_size\n");
 	for (int metric = 0; metric < 3; metric++)
 		for (uint32_t dim : {1u, 2u, 3u, 4u, 5u, 15u, 16u, 17u, 31u, 33u, 63u, 64u, 100u, 127u, 128u, 129u, 300u, 767u, 768u, 769u, 1024u, 1536u, 1999u, 2000u})
-			for (uint32_t maxM : {0u, 2u, 6u, 32u, 64u, 200u})
+			for (uint32_t maxM : {0u, 2u, 6u, 32u, 64u, 200u, 254u, 256u, 258u, 1024u, 1800u, 2036u, 4096u})
 				for (uint32_t ef : {1u, 5u, 64u, 200u, 1000u, 4000u})
 					for (int coop = 0; coop < 2; coop++)
 						for (uint32_t tpr : {4u, 8u})

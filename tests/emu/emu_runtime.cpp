@@ -12,6 +12,7 @@ pthread_mutex_t	   g_mbar_mu = PTHREAD_MUTEX_INITIALIZER;
 int				   g_tma_late = 0;
 int				   g_jitter = 0;
 int				   g_tma_unwaited = 0;
+int				   g_launch_error = 0;
 
 // SIGUSR1 (e.g. `timeout -s USR1`): where every warp of the CTA in flight stands -- for hangs under the emulator
 static Warp *volatile g_live[64];
@@ -131,6 +132,11 @@ void launch(dim3 grid, unsigned block_threads, size_t dyn_smem_bytes, const std:
 {
 	if (g_launch_log.size() < 4096) g_launch_log.emplace_back(block_threads, dyn_smem_bytes);
 	g_launch_count++;
+	if (dyn_smem_bytes > kMaxDynamicSmem)
+	{
+		g_launch_error = 1;  // cudaErrorInvalidValue: the device refuses the launch and runs nothing
+		return;
+	}
 	g_grid_dim = grid;
 	g_block_dim = dim3(block_threads);
 	{

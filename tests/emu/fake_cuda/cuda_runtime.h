@@ -96,6 +96,9 @@ extern pthread_mutex_t	   g_mbar_mu;
 extern int				   g_jitter;	// PGEMB_EMU_JITTER != 0: warps pause at random around atomics (perturbs the interleaving of slots)
 extern int				   g_tma_late;	// set from PGEMB_EMU_TMA at every launch
 extern int				   g_tma_unwaited;	// copies still pending when their CTA exited (late schedule), since load
+extern int				   g_launch_error;	// error of the last launch the runtime refused, until cudaGetLastError() reads it
+// dynamic shared memory a CTA may opt in to on the H100 (227 KB): a larger cudaFuncSetAttribute or launch fails, as on the device
+constexpr size_t		   kMaxDynamicSmem = 232448;
 
 inline Warp &W() { return *tl_warp; }
 inline Lane &L() { return tl_warp->lane[tl_warp->cur]; }
@@ -410,7 +413,12 @@ typedef EmuStream *cudaStream_t;
 typedef EmuEvent  *cudaEvent_t;
 
 static inline const char *cudaGetErrorString(cudaError_t e) { return e == 0 ? "no error" : (e == 2 ? "out of memory" : "invalid value"); }
-static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
+static inline cudaError_t cudaGetLastError()
+{
+	const cudaError_t e = emu::g_launch_error;
+	emu::g_launch_error = cudaSuccess;
+	return e;
+}
 static inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }
 static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDevice(int *d) { *d = 0; return cudaSuccess; }
@@ -457,7 +465,10 @@ static inline cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t = nullptr)
 }
 static inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }
 static inline cudaError_t cudaEventElapsedTime(float *ms, cudaEvent_t a, cudaEvent_t b) { *ms = (float) (b->t_ms - a->t_ms); return cudaSuccess; }
-template <typename F> static inline cudaError_t cudaFuncSetAttribute(F, cudaFuncAttribute, int) { return cudaSuccess; }
+template <typename F> static inline cudaError_t cudaFuncSetAttribute(F, cudaFuncAttribute a, int v)
+{
+	return (a == cudaFuncAttributeMaxDynamicSharedMemorySize && (v < 0 || (size_t) v > emu::kMaxDynamicSmem)) ? cudaErrorInvalidValue : cudaSuccess;
+}
 template <typename F> static inline cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, F, int, size_t) { *n = 1; return cudaSuccess; }
 
 namespace cub {

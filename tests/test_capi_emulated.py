@@ -12,6 +12,8 @@ import subprocess
 import numpy as np
 import pytest
 
+from test_gpu_insert_limits import EFC_CASES
+
 pytestmark = pytest.mark.timeout(1800, method="thread")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -607,3 +609,32 @@ def test_distance_paths_scan(pg, DP, oracle_mod, metric, monkeypatch):
 @pytest.mark.parametrize("metric", ["l2", "cosine", "manhattan"])
 def test_distance_paths_insert(pg, DP, oracle_mod, metric, monkeypatch):
     DP.check_insert(pg, oracle_mod, metric, DP.EMU_INSERT_DIMS, monkeypatch, n=80)
+
+
+@pytest.fixture(scope="module")
+def IL():
+    import test_gpu_insert_limits as il     # GPU tests of the insert path at its size limits: bodies reused below
+    return il
+
+
+@pytest.mark.parametrize("m", [127, 128, 129])
+def test_insert_limits_full_list_replay(pg, IL, oracle_mod, m):
+    """The last few inserts of the m = 127 / 128 / 129 grid builds, replayed from the oracle's records (L2)."""
+    IL.check_full_lists(pg, oracle_mod, m, "l2", 2500, 4, full_build=False)
+
+
+@pytest.mark.parametrize("case", EFC_CASES, ids=[c[0] for c in EFC_CASES])
+def test_insert_limits_efconstruction(pg, IL, oracle_mod, case):
+    """Every bind path at each efConstruction of the ladder, n = 120: the launches' shared memory stays within the opt-in limit."""
+    name, efc, metric = case
+    IL.check_efc(pg, oracle_mod, efc, metric, 120)
+
+
+@pytest.mark.parametrize("metric", ["l2", "cosine", "manhattan"])
+def test_insert_limits_deleted_nodes(pg, IL, oracle_mod, metric):
+    IL.check_deleted(pg, oracle_mod, metric, 300)
+
+
+@pytest.mark.parametrize("metric", ["l2", "cosine", "manhattan"])
+def test_insert_limits_kept_beyond_row_groups(pg, IL, oracle_mod, metric):
+    IL.check_kept_beyond_row_groups(pg, oracle_mod, metric, 200)
